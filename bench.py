@@ -3,12 +3,16 @@
 (BASELINE.json configs[1], "C2").  One "step" = one pass of the hot path (boundary tensors ->
 ingest -> solve -> adjoint -> emit) over one batch of synthetic dense QPs.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--dump-outputs DIR]
 
 * ours      : `value` = device-resident throughput (inputs already in HBM), `e2e` = the same step
               through the reference-facing `_CvxpyLayer.apply` with HOST buffers (H2D + D2H inside
               the timed region).  N > 1: one rank per GPU (torchrun), each rank solves its own
               4096-instance shard (weak scaling), one NCCL gather of solutions + gradients.
+* --dump-outputs DIR : after the timed steps, write what the last device-resident step returned (solutions,
+              status, iteration counts and the gradients in the boundary layout) as DIR/<name>.npy, float64;
+              with N > 1 the shards of all ranks, gathered onto rank 0 (the global batch).
+              Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 * reference : the reference's algorithm on the host cores -- the C oracle (oracle/cone_oracle.c,
               "port": diffcp/SCS are not installable in this image, DESIGN.md) with all threads.
 """
@@ -32,10 +36,10 @@ METRIC = "QP problems/sec fwd+bwd (batch=4096, n=100, m=200, zero+nonneg cones)"
 UNIT = "problems/s"
 # Solver settings shared by both arms (SCS defaults for the forward; LSQR rules of diffcp).
 SOLVER_ARGS = {"eps": 1e-4, "max_iters": 10000, "lsqr_precond": 2, "adaptive_check": 1}
-# DRAM bytes per instance measured by ncu --set full on 296-instance launches (profiles/prof_fwdfast_r1.txt,
-# prof_bwdblk_r1b.txt): fwd_fast_kernel 60.54 MB read + 1.28 MB written; bwd_block_kernel 35.15 MB read
-# (only the live rows of A are staged) + 9.90 MB written back within the launch (the rest sits in L2).
-NCU_DRAM_BYTES_PER_INSTANCE = {"bwd": (35.154432e6 + 9.900288e6) / 296, "fwd": (60.542976e6 + 1.276416e6) / 296}
+# HBM bandwidth of the H100 SXM (NVIDIA data sheet, 700 W card): the denominator of `roofline.frac` unless a measured
+# peak is supplied in MEASURED_PEAKS.json.  Not a rate this benchmark has reached.
+H100_HBM_GBS = 3350.0
+L2_BYTES = 50e6   # H100 L2
 # Algorithmic HBM bytes per instance (SURVEY.md 8d): fwd reads A,P,b,c + writes x,y,s;
 # bwd re-reads data + x,y,s + dx,dy and writes dA,dP,db,dc.
 def algo_bytes(n, m, nnzA, nnzP):
@@ -46,7 +50,7 @@ def algo_bytes(n, m, nnzA, nnzP):
 
 class ClockSampler:
     """Samples SM clocks / throttle reasons DURING the timed region.  Two sources started together: an in-process NVML thread
-    (a sample every 5 ms from the first millisecond -- the timed region of the default run is ~150 ms, less than `nvidia-smi`
+    (a sample every 5 ms from the first millisecond -- the timed region of the default run is a fraction of a second, less than `nvidia-smi`
     sometimes needs to start up) and an `nvidia-smi -lms 100` child as the fallback; `stop()` reports NVML's samples when it has any."""
 
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -122,7 +126,41 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": [f"sampler error: {ex!r}"[:120]], "samples": 0}
 
 
+def device_info(index: int) -> dict:
+    """Name and power limit of the card: an absolute number means little without them."""
+    import torch
+
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        import pynvml as nv  # noqa: PLC0415
+
+        nv.nvmlInit()
+        info["power_limit_w"] = nv.nvmlDeviceGetEnforcedPowerLimit(nv.nvmlDeviceGetHandleByIndex(index)) / 1000.0
+    except Exception:  # noqa: BLE001  (NVML missing: the name alone)
+        pass
+    return info
+
+
 CONFIG = "C2"   # BASELINE.json configs[1] is the headline; the others are parity-test cases that can be timed too
+DUMP_BUDGET_BYTES = 60_000_000   # --dump-outputs writes at most this much (64 MB less headroom for the .npy headers)
+
+
+def dump_outputs(dirname: str, arrays: dict, B: int) -> None:
+    """Writes `arrays` (name -> (tensor, batch axis)) as float64 .npy files.  When the whole batch would exceed
+    DUMP_BUDGET_BYTES, a fixed sample of instances (seeded, the same for every array and every run) is written instead,
+    and `instances.npy` lists which ones."""
+    import torch
+
+    per_instance = sum(8 * t.numel() // max(t.shape[ax], 1) for t, ax in arrays.values() if t is not None)
+    k = int(min(B, DUMP_BUDGET_BYTES // max(per_instance, 1)))
+    idx = np.arange(B) if k >= B else np.sort(np.random.default_rng(0).choice(B, k, replace=False))
+    os.makedirs(dirname, exist_ok=True)
+    np.save(os.path.join(dirname, "instances.npy"), idx.astype(np.float64))
+    for name, (t, ax) in arrays.items():
+        if t is None:
+            continue
+        sel = t.index_select(ax, torch.as_tensor(idx, device=t.device)) if k < B else t
+        np.save(os.path.join(dirname, f"{name}.npy"), sel.detach().to(torch.float64).cpu().numpy())
 
 
 def make_workload(batch: int, seed: int):
@@ -142,7 +180,7 @@ def config_block(bt, B: int, world: int, l2: str) -> dict:
 
 def l2_note(st, B: int) -> str:
     nbytes = (st.nnzA + st.m + st.n + 1 + st.nnzP) * B * 8
-    return f"inputs ({nbytes / 1e9:.2f} GB/step) vs 126 MB L2" + ("" if nbytes > 130e6 else "; NOT larger than L2 (secondary config, no flush)")
+    return f"inputs ({nbytes / 1e9:.2f} GB/step) vs {L2_BYTES / 1e6:.0f} MB L2" + ("" if nbytes > L2_BYTES else "; NOT larger than L2 (secondary config, no flush)")
 
 
 def host_cores() -> int:
@@ -514,7 +552,7 @@ def run_ours(a):
         ms_strong, _, _, _ = timed_sharded(Bs, a.chunk)
         strong = {"global_batch": Bs * world, "batch_per_gpu": Bs, "ms_per_step": ms_strong, "value": Bs * world / (ms_strong * 1e-3), "unit": UNIT,
                   "chunks_per_gpu": len(chunk_list(Bs, a.chunk)),
-                  "note": f"{Bs} instances per GPU = {Bs / 148:.2f} waves of one CTA per SM: wave quantisation and the fixed per-launch costs bound strong scaling"}
+                  "note": f"{Bs} instances per GPU = {Bs / torch.cuda.get_device_properties(dev).multi_processor_count:.2f} waves of one CTA per SM: wave quantisation and the fixed per-launch costs bound strong scaling"}
         if a.verify_exchange:
             # every slot of rank 0's buffer against an NCCL gather of the same tensors
             ok = True
@@ -530,13 +568,17 @@ def run_ours(a):
             if rank == 0:
                 print(f"[bench] exchange verified against NCCL gather: {ok} (p2p={xchg.p2p})", file=sys.stderr)
                 assert ok
+    # what the last timed step returned (written out at the end, after every timed measurement)
+    gA_ev, gq_ev, gP_ev = (bufs["gA_eval"], bufs["gq_eval"], bufs["gP_eval"]) if world > 1 else dbuf["ev"]
+    last_step = {"x": (sol.x, 0), "y": (sol.y, 0), "s": (sol.s, 0), "status": (sol.status, 0), "iters": (sol.iters, 0),
+                 "lsqr_iters": (its, 0), "dA_eval": (gA_ev, 1), "dq_eval": (gq_ev, 1), "dP_eval": (gP_ev, 1)}
     status = sol.status.cpu().numpy()
     iters = sol.iters.cpu().numpy()
     lits = its.cpu().numpy()
     n_fallback = eng.fallback_count()   # block solver -> equilibrated LSQR fallbacks of the last backward (-1: block solver not in use)
 
     # ---- end-to-end through the reference-facing call with HOST buffers ----
-    # Warm-up with the same object lifetimes as the timed loop.  The first two calls pay ~360 ms each for the pinned
+    # Warm-up with the same object lifetimes as the timed loop.  The first two calls pay for allocating the pinned
     # result buffers (two generations are alive at a time); at least three steady steps follow them before timing.
     e2e_warm = max(5, a.warmup + 2)
     for _ in range(e2e_warm):
@@ -568,17 +610,17 @@ def run_ours(a):
             step_e2e(True)
         sync()
         tw = time.perf_counter()
-        for _ in range(3):
+        for _ in range(n_e2e):
             step_e2e(True)
         sync()
-        e2e_pageable = {"value": Btot / ((time.perf_counter() - tw) / 3), "unit": UNIT, "steps": 3,
+        e2e_pageable = {"value": Btot / ((time.perf_counter() - tw) / n_e2e), "unit": UNIT, "steps": n_e2e,
                         "note": "pageable host inputs (the reference's CPU tensors): batch slices gathered into a ring of pinned staging buffers by a background thread, then the same two-stream pipeline"}
         del pA, pq, pP
     # f1 + f2 in one number: only parameters cross PCIe, the matrices are constants of the layer
     e2e_fused = None
     if world == 1 and CONFIG == "C2" and rank == 0:
         try:
-            e2e_fused = fused_param_variant(bt, B, dev, SOLVER_ARGS, max(3, min(a.steps, 10)), a.warmup)
+            e2e_fused = fused_param_variant(bt, B, dev, SOLVER_ARGS, n_e2e, a.warmup)
         except Exception as ex:  # noqa: BLE001  (a secondary measurement must not take the line down)
             e2e_fused = {"error": repr(ex)[:300]}
     npel = hP.numel() if hP is not None else 0
@@ -592,7 +634,7 @@ def run_ours(a):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:  # noqa: BLE001
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
         dom = "bwd" if kt["bwd"] >= kt["fwd"] else "fwd"
         dom_bytes = (bwd_b if dom == "bwd" else fwd_b) * B
         ach = dom_bytes / (kt[dom] * 1e-3) / 1e9
@@ -601,17 +643,18 @@ def run_ours(a):
             ns = min(a.cpu_sample, B)
             if CONFIG == "C4":   # the oracle's dense 1000 x 1000 factor makes an instance a multi-second job per core
                 ns = min(ns, 128)
-            v, dtc, cores, solved_c, per = cpu_arm(bt, ns, 1 if CONFIG == "C4" else 2, 0 if CONFIG == "C4" else 1, spread=True)
+            cpu_warm = 0 if CONFIG == "C4" else 1
+            v, dtc, cores, solved_c, per = cpu_arm(bt, ns, a.steps, cpu_warm, spread=True)
             cpu = {"value": v, "unit": UNIT, "cores": cores, "kind": "port",
-                   "sample": f"first {ns} instances of the same batch, {0 if CONFIG == 'C4' else 1} warm-up + {1 if CONFIG == 'C4' else 2} timed passes ({dtc:.2f} s each), oracle/cone_oracle.c with OpenMP over instances",
+                   "sample": f"first {ns} instances of the same batch, {cpu_warm} warm-up + {a.steps} timed passes ({dtc:.2f} s each), oracle/cone_oracle.c with OpenMP over instances",
                    "ms_per_pass": [round(x, 1) for x in per]}
         info = eng.kernel_info()
         line = {"metric": METRIC, "value": Btot / (ms_step * 1e-3), "unit": UNIT, "n_gpus": world, "steps": a.steps,
                 "warmup": a.warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "f64", "data": "synthetic",
                 "config": config_block(bt, B, world, l2_note(st, B)),
-                # value = mean over exactly `steps` timed steps (the contract's definition).  The per-step wall times and
-                # their median are diagnostics only: on shared boxes single steps sometimes take 2x (profiles/README.md).
+                # value = mean over exactly `steps` timed steps.  The per-step wall times and their median are diagnostics
+                # only: on a host shared with other work single steps sometimes take twice as long.
                 "e2e": {"value": Btot / (ms_e2e * 1e-3), "unit": UNIT, "ms_per_step": ms_e2e,
                         "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h), "warmup_steps": e2e_warm,
                         "diagnostic_wall_ms_per_step": [round(v, 1) for v in per_step],
@@ -622,19 +665,29 @@ def run_ours(a):
                 **({"strong_scaling": strong, "exchange": {"kind": "peer-to-peer copy engines (CUDA IPC over NVLink), chunked behind the solve" if xchg.p2p else "NCCL gather into preallocated slots",
                                                           "bytes_per_rank": int(slot_bytes), "chunk": a.chunk, "numa_bound": bool(numa_bound)}} if world > 1 else {}),
                 "roofline": {"bound": "hbm", "kernel": eng.path_info()[dom], "achieved": ach, "peak": peak, "unit": "GB/s",
-                             "frac": ach / peak, "traffic": (NCU_DRAM_BYTES_PER_INSTANCE.get(dom, 0) * B / 1e9 or None) if CONFIG == "C2" else None,
-                             "traffic_unit": "GB per launch (ncu dram__bytes_read+write per instance, profiles/prof_*_r1*.txt, x B)",
-                             "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 GB/s",
+                             "frac": ach / peak, "traffic": None, "traffic_unit": "GB per launch (not measured on the H100)",
+                             "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else f"H100 SXM data sheet {H100_HBM_GBS:.0f} GB/s",
                              "note": "on-chip iterative solve: HBM is touched once in/out per instance, the loop runs in shared memory"},
                 "kernel_ms": {k: round(v, 3) for k, v in kt.items()},
                 "kernel_geometry": info, "kernel_paths": eng.path_info(),
                 "solver": {"solved": int((status == 1).sum()), "of": int(status.size), "fwd_iters_mean": float(iters.mean()),
                            "fwd_iters_max": int(iters.max()), "lsqr_iters_mean": float(lits.mean()), "lsqr_iters_max": int(lits.max()),
                            "lsqr_fallback": n_fallback, "lsqr_fallback_of": int(lits.size)},
-                "clocks": clocks}
+                "clocks": clocks, "device": device_info(local)}
         if cpu:
             line["cpu_baseline"] = cpu
         print(json.dumps(line))
+    if a.dump_outputs:
+        if world > 1:   # the caller of the sharded path receives every rank's shard: gather them onto rank 0 along the batch axis
+            for name, (t_, ax) in list(last_step.items()):
+                if t_ is None:
+                    continue
+                t_ = t_.contiguous()
+                parts = [torch.empty_like(t_) for _ in range(world)] if rank == 0 else None
+                dist.gather(t_, parts, dst=0)
+                last_step[name] = (torch.cat(parts, dim=ax) if rank == 0 else None, ax)
+        if rank == 0:
+            dump_outputs(a.dump_outputs, last_step, Btot)
     if world > 1:
         dist.destroy_process_group()
 
@@ -652,6 +705,8 @@ def main():
                    help="workload (default: the headline C2; others are secondary measurements)")
     p.add_argument("--chunk", type=int, default=1024, help="N > 1: instances per pipeline chunk (results of a chunk travel to rank 0 behind the next chunk's solve)")
     p.add_argument("--verify-exchange", action="store_true", help="N > 1: check rank 0's gathered buffer against an NCCL gather")
+    p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                   help="after the timed steps, write the outputs of the last step as DIR/<name>.npy (float64, at most 64 MB)")
     p.add_argument("--set", action="append", default=[], metavar="KEY=VALUE",
                    help="override a solver argument for both arms, e.g. --set acceleration_lookback=0")
     a = p.parse_args()

@@ -1,7 +1,7 @@
 """ctypes binding of libbcone.so (the C ABI declared in include/bcone.h).
 
 There is no CPU fallback: if the CUDA library is missing or no CUDA device is present the
-engine raises.  The library is built in-tree by ``cvxpylayers_b200.build`` (nvcc, sm_100a).
+engine raises.  The library is built in-tree by ``cvxpylayers_b200.build`` (nvcc, sm_90a).
 """
 from __future__ import annotations
 
@@ -54,7 +54,7 @@ def load() -> C.CDLL:
         return _lib
     if not LIB_PATH.exists():
         raise EngineUnavailable(
-            f"{LIB_PATH} not found: build it with `python -m cvxpylayers_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python -m cvxpylayers_b200.build` (nvcc, sm_90a). "
             "The engine has no CPU or PyTorch fallback.")
     try:
         lib = C.CDLL(str(LIB_PATH))

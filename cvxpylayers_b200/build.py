@@ -1,7 +1,9 @@
-"""Builds libbcone.so (the C-ABI CUDA library) in-tree for sm_100a with nvcc.
+"""Builds libbcone.so (the C-ABI CUDA library) in-tree for the H100 (sm_90a) with nvcc.
 
 Run as ``python -m cvxpylayers_b200.build``; ``__graft_entry__.build()`` calls :func:`build`.
-nvcc cross-compiles without a GPU; the resulting .so travels to the GPU box with the tree.
+nvcc cross-compiles without a GPU.  The translation units share no device symbols, so each is
+compiled on its own (in parallel, into a temporary directory) and the objects are linked into one
+shared library.
 """
 from __future__ import annotations
 
@@ -9,6 +11,8 @@ import os
 import shutil
 import subprocess
 import sys
+import tempfile
+from concurrent.futures import ThreadPoolExecutor
 from pathlib import Path
 
 PKG = Path(__file__).resolve().parent
@@ -16,8 +20,8 @@ CSRC = PKG / "csrc"
 SOURCES = ["api.cu", "fwd.cu", "fwd_fast.cu", "bwd.cu", "bwd_fast.cu", "bwd_block.cu", "pack.cu"]
 HEADERS = [CSRC / "common.cuh", PKG.parent / "include" / "bcone.h"]
 LIB = PKG / "libbcone.so"
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
-              "-Xcompiler", "-fPIC", "-shared"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*ARCH_FLAGS, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def _nvcc() -> str:
@@ -39,15 +43,24 @@ def build(force: bool = False, verbose: bool = False, defines: tuple = (), out: 
     target = Path(out) if out else LIB
     if not force and not defines and not out and not stale():
         return LIB
-    cmd = [_nvcc(), *NVCC_FLAGS, *defines, "-o", str(target), *[str(CSRC / s) for s in SOURCES]]
-    if verbose:
-        cmd.insert(1, "-Xptxas=-v")
-    env = dict(os.environ)
-    r = subprocess.run(cmd, capture_output=True, text=True, env=env)
-    if r.returncode != 0:
-        raise RuntimeError("nvcc failed:\n" + r.stdout + r.stderr)
-    if verbose:
-        print(r.stderr)
+    nvcc = _nvcc()
+    with tempfile.TemporaryDirectory(prefix="bcone_build_") as td:
+        objs = [os.path.join(td, Path(s).stem + ".o") for s in SOURCES]
+
+        def compile_one(src_obj):
+            src, obj = src_obj
+            cmd = [nvcc, *NVCC_FLAGS, *(["-Xptxas=-v"] if verbose else []), *defines, "-c", "-o", obj, str(CSRC / src)]
+            return subprocess.run(cmd, capture_output=True, text=True)
+
+        with ThreadPoolExecutor(max_workers=max(1, min(len(SOURCES), os.cpu_count() or 1))) as ex:
+            results = list(ex.map(compile_one, zip(SOURCES, objs)))
+        link = subprocess.run([nvcc, *ARCH_FLAGS, "-shared", "-o", str(target), *objs], capture_output=True, text=True) \
+            if all(r.returncode == 0 for r in results) else None
+        for r in [*results, *([link] if link else [])]:
+            if r.returncode != 0:
+                raise RuntimeError("nvcc failed:\n" + r.stdout + r.stderr)
+            if verbose:
+                print(r.stderr)
     return target
 
 

@@ -68,8 +68,8 @@ struct Handle {
   int tma_ok = 0, psd_total = 0, p_in_smem = 0;
   int fwd_indirect = 0, bwd_vec_global = 0;   // large instances: CG instead of Cholesky, vectors in a global slab
   // <= 256-thread instances have a second build of the generic kernels for four resident CTAs per SM (64 registers).  It wins
-  // when the batch exceeds what the 128-register build keeps resident (more CTAs overlap each other's stalls: exp-cone workload
-  // +24 %) and loses when every instance is resident anyway and only its own latency counts (SDP at B = 256: -25 %), so the
+  // when the batch exceeds what the 128-register build keeps resident (more CTAs overlap each other's stalls: exp-cone workload)
+  // and loses when every instance is resident anyway and only its own latency counts (SDP at B = 256), so the
   // choice is made per launch from the batch size.  BCONE_SMALL_CTA=0 disables, =2 forces.
   int fwd_small = 0, bwd_small = 0, fwd_ctas_small = 0, bwd_ctas_small = 0, small_mode = 1;
   int fwd_factor_global = 0;                  // in between: values on chip, vectors + packed Cholesky factor in the slab (direct solve from L2 / HBM)
@@ -230,9 +230,9 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
         size_t sm = bc_fwd_smem_bytes(n, m, d->nnzA, tt, max_psd, ind, d->ns, d->ep + d->ed);
         if (sm <= smem_cap) {
           h->fwd_threads = tt; h->fwd_smem = sm; h->fwd_indirect = ind;
-          // (n <= 512: one thread per column in the transposed triangular product; measured on the sparse LP with n = 1000 the
-          //  slab mode streams 8 MB of factor per iteration and CTA from HBM and loses to conjugate gradients, 12.6 s vs 5.8 s per
-          //  512-batch, while at n = 101 it wins 37x)
+          // (n <= 512: one thread per column in the transposed triangular product; on the sparse LP with n = 1000 the slab mode
+          //  streams 8 MB of factor per iteration and CTA from HBM and loses to conjugate gradients, while at n = 101 the factor
+          //  stays in L2 and the slab mode wins by a wide margin)
           if (ind && !force_indirect && n <= 512) { h->fwd_indirect = 0; h->fwd_factor_global = 1; }
           return true;
         }

@@ -1,5 +1,5 @@
 // common.cuh -- device-side building blocks shared by the forward (fwd.cu) and backward
-// (bwd.cu) kernels of the batched cone engine.  sm_100a only.
+// (bwd.cu) kernels of the batched cone engine.  sm_90a (H100) only.
 //
 // Execution model: ONE CTA PER PROBLEM INSTANCE, persistent CTAs pulling instance ids from a
 // global atomic counter (iteration counts vary 10x across a batch, a static grid would leave
@@ -411,7 +411,7 @@ __device__ __forceinline__ double butterfly4(double a0, double a1, double a2, do
 
 // FP64 tensor-core tile product D(8x8) += A(8x4) * B(4x8), one warp (SASS: DMMA.8x8x4).  Fragment layout
 // (PTX mma.m8n8k4.f64): lane holds A[lane >> 2][lane & 3], B[lane & 3][lane >> 2] and the two accumulator
-// entries D[lane >> 2][2 (lane & 3) + {0, 1}].  There is no tcgen05 kind for f64; this is the tensor path the
+// entries D[lane >> 2][2 (lane & 3) + {0, 1}].  wgmma has no f64 kind; this is the Hopper tensor path the
 // dense fp64 set-up phases (K formation, Cholesky trailing update, W = L^{-1} A', S = W W') run on.
 __device__ __forceinline__ void dmma884(double &d0, double &d1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));

@@ -1,7 +1,7 @@
 // fwd_fast.cu -- forward solve for dense A with polyhedral cones (zero + nonneg rows): the same operator
 // splitting as fwd.cu (same formulas, same termination rules; SURVEY.md 8a F3-F6, the work diffcp/SCS do
 // at src/cvxpylayers/interfaces/diffcp_if.py:365,369), re-laid out around what the shared-memory
-// micro-benchmarks showed (tools/microbench.cu, profiles/README.md): the per-iteration products with A were
+// micro-benchmarks of tools/microbench.cu showed: the per-iteration products with A were
 // bound by shared-memory bandwidth and shuffle throughput, not by FP64 issue.
 //
 //   * A LIVES IN REGISTERS: thread (R, C) of the 512 keeps the 4 x 10 tile A[4R..4R+3, 10C..10C+9] of the
@@ -57,7 +57,7 @@ struct Geo {
   // (10 tiles per row, 8 lanes per quarter); with 16-byte units u = KR R kst / 2 + 5 C + c / 2 the two halves collide unless
   // KR kst / 2 = 2 (mod 8): stride 100 costs 60 % extra wavefronts on the 80 KB that every iteration reads, 106 none.
   // (Compile-time geometries only: in the runtime-geometry instantiation one more loop-invariant value pushed the tile products of
-  //  the iteration loop into local memory, +6-9 % per solve measured, more than the conflicts cost.)
+  //  the iteration loop into local memory, which costs more than the conflicts do.)
   __host__ __device__ __forceinline__ int kst() const { return (CT_ != 0 && KR() == 2) ? npad() + ((10 - (npad() & 7)) & 7) : npad(); }
   __host__ __device__ __forceinline__ int oXC() const { return npad() * kst(); }
   __host__ __device__ __forceinline__ int szPart() const { const int a = RTu() * npad(), b = rowsR() * CT(); return ((a > b ? a : b) + 1) & ~1; }
@@ -469,7 +469,7 @@ __device__ __noinline__ void check_tail(const FwdArgs &a, double *vx, double *vy
 }
 
 // Column maxima of |P^| for one Ruiz pass: four lanes per index over the packed symmetric matrix, folded into tn.
-// (A variant with separate row / column walks, running addresses and the factor e_j applied once measured 15 % slower:
+// (A variant with separate row / column walks, running addresses and the factor e_j applied once was slower:
 // the pass is bound by the dependent max chain of each lane, not by the index arithmetic.)
 __device__ __noinline__ void ruiz_P_part(const double *Pl, const double *En, double *tn, int n) {
   const int t = threadIdx.x, q = t & 3;
@@ -954,7 +954,7 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
           // The callee chain needs more registers than the tile leaves free.  Parking the tile in the slab for the
           // duration of the call (128 KB per CTA, L2) keeps it out of the call's live set, so the register allocation
           // of the iteration loop is the one without acceleration; the compiler's own answer was to keep a third of
-          // the tile in local memory for the whole loop (+20 % per iteration, measured).
+          // the tile in local memory for the whole loop, which slows every iteration.
           double *park = a.park + (size_t)blockIdx.x * (TR * TCR * FT) + t;
 #pragma unroll
           for (int r = 0; r < TR; r++)

@@ -1,4 +1,4 @@
-"""Drop-in solver interface: the B200 twin of ``cvxpylayers/interfaces/diffcp_if.py``.
+"""Drop-in solver interface (solver name "B200"): the GPU twin of ``cvxpylayers/interfaces/diffcp_if.py``.
 
 Mirrors, name for name and argument for argument, what the reference's torch layer expects of a
 backend (SURVEY.md section 8b):

@@ -198,7 +198,7 @@ def dense_lp(B: int, n: int, m: int, seed: int = 0) -> Batch:
 
 def qp_as_socp(bt: Batch) -> Batch:
     """The same QPs in the form the reference's DIFFCP path hands over: DIFFCP cannot take a quadratic objective
-    (``/root/reference/src/cvxpylayers/_quad_form_dpp.py:29-32``: "DIFFCP decomposes quad_form to SOC"), so cvxpy
+    (``src/cvxpylayers/_quad_form_dpp.py:29-32``: "DIFFCP decomposes quad_form to SOC"), so cvxpy
     canonicalises ``1/2 x'Px`` with ``P = R'R`` through an epigraph variable and one second-order cone of size n + 2,
 
         min c'x + t   s.t.  (original rows),   (t + 1, t - 1, sqrt2 R x) in SOC     [<=> x'Px <= 2t],

@@ -1,5 +1,5 @@
 /*
- * bcone.h -- C ABI of the B200-native batched cone-program solve-and-differentiate
+ * bcone.h -- C ABI of the H100-native batched cone-program solve-and-differentiate
  * engine (libbcone.so).  Plain pointers and sizes only; every data pointer is the
  * CALLER'S DEVICE MEMORY unless stated, every call is asynchronous on the given
  * CUDA stream, every function returns 0 on success and a negative code on error

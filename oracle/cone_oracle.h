@@ -2,7 +2,7 @@
  * cone_oracle.h -- CPU ORACLE (TEST INFRASTRUCTURE, NOT PRODUCT CODE).
  *
  * Plain-C, fp64 restatement of the hot path the reference delegates to
- * diffcp 1.1.4 + SCS 3.2.9 (neither is vendored in /root/reference nor
+ * diffcp 1.1.4 + SCS 3.2.9 (neither is vendored in the reference nor
  * installable here, see DESIGN.md "Oracle"):
  *   forward : diffcp.solve_and_derivative_batch  (reference call site
  *             src/cvxpylayers/interfaces/diffcp_if.py:365, :369)

@@ -78,20 +78,22 @@ def test_cached_setup_is_the_uncached_algorithm(cuda_device, shape):
 
 
 def test_cached_setup_without_quadratic_term(cuda_device):
-    """An LP of the register-tiled shape (no P): the cached path has nothing to load but Kinv."""
+    """An LP of the register-tiled shape (no P): the cached path has nothing to load but Kinv.  (90 x 170: the tile grid
+    keeps at least half of the CTA's threads busy, which the register-tiled kernel requires.)"""
     B, dev = 48, cuda_device
-    bt = pr.dense_qp(B, 60, 160, 20, seed=4, with_P=False)
+    bt = pr.dense_qp(B, 90, 170, 20, seed=4, with_P=False)
     st = bt.structure
     eng = Engine(st, dev)
+    assert "register-tiled" in eng.path_info()["fwd"]
     A, b, c = _t(bt.A_vals, dev), _t(bt.b, dev), _t(bt.c, dev)
     S = make_settings(dict(eps=1e-6, max_iters=200000))
     cache = eng.new_cache(B)
-    if cache is None:
-        pytest.skip("this LP shape does not run the register-tiled kernel")
+    assert cache is not None and cache.numel() * 8 == eng.cache_bytes(B)
     one = eng.solve(A, b, c, None, S, cache=cache, reuse=False)
     two = eng.solve(A, b, c, None, S, warm=one, cache=cache, reuse=True)
     ref = eng.solve(A, b, c, None, S, warm=one)
     hdr = cache.view(B, -1)[:, 0].cpu().numpy()
+    assert (hdr == S.scale).any()
     ki = torch.tensor(np.nonzero(hdr == S.scale)[0], device=dev)
     assert torch.equal(two.x[ki], ref.x[ki]) and torch.equal(two.iters[ki], ref.iters[ki])
 

@@ -9,6 +9,7 @@ from cvxpylayers_b200.engine import Engine, make_settings
 
 dev = torch.device("cuda", 0)
 B = 4096
+sms = torch.cuda.get_device_properties(dev).multi_processor_count   # one resident instance per SM
 args = make_settings({"eps": 1e-4, "max_iters": 10000, "adaptive_check": 1})
 t = lambda a: None if a is None else torch.as_tensor(a, dtype=torch.float64, device=dev)
 for (n, m, z) in [(100, 200, 50), (90, 200, 40), (100, 190, 50), (80, 160, 40), (96, 192, 48)]:
@@ -26,5 +27,5 @@ for (n, m, z) in [(100, 200, 50), (90, 200, 40), (100, 190, 50), (80, 160, 40), 
     its = float(sol.iters.float().mean())
     print(json.dumps({"n": n, "m": m, "z": z, "kernel": eng.path_info()["fwd"], "geometry": "compile-time <10,50>" if (n, m) == (100, 200) else "runtime <0,0>",
                       "fwd_ms_per_4096": round(ms, 3), "iters_mean": round(its, 2), "solved": int((sol.status == 1).sum()),
-                      "us_per_instance": round(ms * 1e3 * 148 / B, 1), "us_per_instance_iteration": round(ms * 1e3 * 148 / B / its, 3),
+                      "us_per_instance": round(ms * 1e3 * sms / B, 1), "us_per_instance_iteration": round(ms * 1e3 * sms / B / its, 3),
                       "flops_scale_vs_100x200": round(n * m / 20000, 3)}))

@@ -1,5 +1,5 @@
 // Micro-benchmarks of the shared-memory matvec building blocks (cycles per call, one CTA per SM).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench tools/microbench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench tools/microbench.cu
 #include <cstdio>
 #include <vector>
 #define BC_CHOLPROF 1
@@ -336,7 +336,8 @@ int main() {
   cudaMemset(a.cyc, 0, sizeof(unsigned long long) * NT);
   const size_t smem = sizeof(double) * (m * n + n * (n + 1) / 2 + 2 + n + m + m + n + 20 * n + 256);
   cudaFuncSetAttribute(mb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  const int grid = 148;
+  int grid = 0;   // one CTA per SM
+  cudaDeviceGetAttribute(&grid, cudaDevAttrMultiProcessorCount, 0);
   mb_kernel<<<grid, 512, smem>>>(a);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaDeviceSynchronize();

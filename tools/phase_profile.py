@@ -23,10 +23,12 @@ sol = eng.solve(A, b, c, P, args); eng.vjp(A, b, c, sol.x, sol.y, sol.s, dx, dy,
 out = (C.c_uint64 * 32)()
 eng.lib.bcone_set_profile(eng.h, 1, out)
 v = np.array(list(out), dtype=np.float64) / B   # cycles per instance
+MHZ = torch.cuda.clock_rate(0)   # SM clock over the last sample period, read right after the profiled calls
+print(torch.cuda.get_device_name(0), "SM clock", MHZ, "MHz")
 names = {5: "  [chol P] factor", 6: "  [chol P] inverse", 16: "  [eq] A sweep", 17: "  [eq] P part", 18: "  [eq] scale update",
          19: "  [K] A'RA", 20: "  [K] + P", 21: "  [K] chol+inv", 22: "  [K] g", 23: "  [it] A'w", 24: "  [it] Li rows", 25: "  [it] Li cols",
          26: "  [it] A p", 27: "  [it] reduce", 28: "  [it] update+proj", 0: "fwd load", 1: "fwd equilibration", 2: "fwd K+chol+inv+g", 3: "fwd iterations", 4: "fwd checks",
          8: "bwd load", 9: "bwd Px + chol/inv P", 10: "bwd W", 11: "bwd S", 12: "bwd chol/inv S", 13: "bwd q+LSQR", 14: "bwd solve+write"}
 for k, nm in names.items():
-    print(f"{nm:26s} {v[k]:10.0f} cycles/instance  {v[k] / 1.965e3:7.1f} us")
-print("fwd total us", v[:5].sum() / 1.965e3, "bwd total us", v[8:15].sum() / 1.965e3, "iters", sol.iters.float().mean().item())
+    print(f"{nm:26s} {v[k]:10.0f} cycles/instance  {v[k] / MHZ:7.1f} us")
+print("fwd total us", v[:5].sum() / MHZ, "bwd total us", v[8:15].sum() / MHZ, "iters", sol.iters.float().mean().item())

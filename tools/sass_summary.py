@@ -1,7 +1,7 @@
-"""Per-kernel SASS evidence for the shipped library: counts of the instructions that prove the Blackwell paths are in
+"""Per-kernel SASS evidence for the shipped library: counts of the instructions that prove the Hopper paths are in
 the binary (UBLKCP = cp.async.bulk / TMA, SYNCS = mbarrier, DMMA = FP64 tensor-core mma, plus DFMA / LDS / STS / BAR / RED /
-local-memory spills), the arch of the cubin and the hash of the .so, so that profiles/ ties the measured binary to the
-sources.     python tools/sass_summary.py > profiles/sass_summary_r2.txt"""
+local-memory spills), the arch of the cubin and the hash of the .so, so that a stored profile ties the measured binary to the
+sources.     python tools/sass_summary.py > sass_summary.txt"""
 import hashlib, os, re, subprocess, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

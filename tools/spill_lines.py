@@ -7,10 +7,12 @@ of local memory".  Compiles one .cu of csrc/ to a cubin with -lineinfo, disassem
 import collections, os, re, subprocess, sys, tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from cvxpylayers_b200.build import ARCH_FLAGS  # noqa: E402
 src, sub, defs = sys.argv[1], sys.argv[2], [a for a in sys.argv[3:] if a.startswith("-D")]
 with tempfile.TemporaryDirectory() as td:
     cub = os.path.join(td, "k.cubin")
-    r = subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xptxas=-v", *defs, "-cubin", "-o", cub,
+    r = subprocess.run(["nvcc", *ARCH_FLAGS, "-lineinfo", "-O3", "-std=c++17", "-Xptxas=-v", *defs, "-cubin", "-o", cub,
                         os.path.join(ROOT, "cvxpylayers_b200", "csrc", src)], capture_output=True, text=True)
     if r.returncode:
         sys.exit(r.stderr)
