@@ -29,6 +29,9 @@ size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int t
 cudaError_t bc_bwd_configure(int dense, size_t smem, int small_cta);
 cudaError_t bc_bwd_occupancy(int dense, int threads, size_t smem, int *ctas, int small_cta);
 cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st, int small_cta);
+cudaError_t bc_jvp_configure(int dense, size_t smem, int small_cta);
+cudaError_t bc_jvp_occupancy(int dense, int threads, size_t smem, int *ctas, int small_cta);
+cudaError_t bc_jvp_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st, int small_cta);
 size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads);
 cudaError_t bc_bwdf_configure(int n, size_t smem);
 cudaError_t bc_bwdf_occupancy(int n, int threads, size_t smem, int *ctas);
@@ -76,12 +79,16 @@ struct Handle {
   size_t fwd_ws_stride = 0, bwd_ws_stride = 0;
   // Per-stream scratch slabs (one per CTA of the grid): launches on different streams may overlap, launches on one
   // stream cannot, so the stream is the unit of ownership.  Allocated on first use.
-  struct StreamWs { cudaStream_t s; double *fwd = nullptr, *bwd = nullptr, *aa = nullptr, *park = nullptr; size_t aa_cap = 0; };
+  struct StreamWs { cudaStream_t s; double *fwd = nullptr, *bwd = nullptr, *aa = nullptr, *park = nullptr, *jvp = nullptr; size_t aa_cap = 0; };
   std::vector<StreamWs> sws;
   int block_bwd = 0, blk_threads = 0; size_t blk_smem = 0;   // KKT-block preconditioned backward (lsqr_precond = 2)
   int *fail_list[RING] = {nullptr}; int fail_cap[RING] = {0};
   int fast_fwd = 0;  // dense A, polyhedral cones, direct mode: register-tiled forward (fwd_fast.cu)
   int fast_bwd = 0;  // dense A, polyhedral cones, dense-or-no P: fused single-pass backward (bwd_fast.cu)
+  // forward-mode derivative (bcone_jvp): always the generic kernel (bwd.cu, JVP = true), so structures on the fused backward
+  // need a generic geometry of their own; chosen by the same rule as the generic backward's.  jvp_ok = 0: none fits.
+  int jvp_ok = 0, jvp_threads = 0, jvp_p_in_smem = 0, jvp_vec_global = 0, jvp_ctas = 0, jvp_small = 0, jvp_ctas_small = 0;
+  size_t jvp_smem = 0, jvp_ws_stride = 0;
   long long launches = 0;
   int last_block_slot = -1;   // ring slot of the last block-preconditioned vjp (its fallback counter is read by bcone_fallback_count)
   unsigned long long *prof = nullptr;   // device [32] phase cycle counters (bcone_set_profile)
@@ -239,16 +246,18 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
       }
     return false;
   };
-  auto pick_bwd = [&]() -> bool {   // prefer P staged in shared memory, then vectors on chip, then vectors in L2
+  // generic LSQR kernel (bwd.cu): prefer P staged in shared memory, then vectors on chip, then vectors in L2
+  auto pick_generic = [&](int &g_threads, size_t &g_smem, int &g_p_in_smem, int &g_vec_global) -> bool {
     for (int vg = 0; vg <= 1; vg++)
       for (int psm = (S.nnzP > 0 ? 1 : 0); psm >= 0; psm--)
         for (int tt = threads; tt >= 64; tt /= 2) {
           size_t sm = bc_bwd_smem_bytes(n, m, npoly, d->nnzA, psm ? S.nnzP : 0, tt, max_psd, psd_total, d->ep + d->ed, vg);
-          if (sm <= smem_cap) { h->bwd_threads = tt; h->bwd_smem = sm; h->p_in_smem = psm; h->bwd_vec_global = vg; return true; }
+          if (sm <= smem_cap) { g_threads = tt; g_smem = sm; g_p_in_smem = psm; g_vec_global = vg; return true; }
           if (psm) break;  // do not trade threads for P residency
         }
     return false;
   };
+  auto pick_bwd = [&]() -> bool { return pick_generic(h->bwd_threads, h->bwd_smem, h->p_in_smem, h->bwd_vec_global); };
   // fast backward path: same launch geometry fields, different kernel
   if (S.dense && S.ncones == 0 && d->ep + d->ed == 0 && n <= 128 && (n % 2) == 0 && (S.nnzP == 0 || S.p_dense)) {
     for (int tt = threads; tt >= 64; tt /= 2) {
@@ -304,6 +313,17 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
   if (h->fwd_indirect || h->fwd_factor_global) h->fwd_ws_stride = bc_fwd_ws_doubles(n, m, h->fwd_factor_global);
   if (h->bwd_vec_global && !h->fast_bwd) h->bwd_ws_stride = bc_bwd_ws_doubles(n, m, npoly);
   h->tma_ok = (d->nnzA > 0 && (d->nnzA % 2) == 0 && (size_t)d->nnzA * 8 < (1u << 20)) ? 1 : 0;
+  // forward-mode derivative: the generic geometry (the backward's own when the backward is generic).  A structure without
+  // one is still accepted; only bcone_jvp refuses it.
+  if (pick_generic(h->jvp_threads, h->jvp_smem, h->jvp_p_in_smem, h->jvp_vec_global) && bc_jvp_configure(S.dense, h->jvp_smem, 0) == cudaSuccess) {
+    h->jvp_ok = 1;
+    bc_jvp_occupancy(S.dense, h->jvp_threads, h->jvp_smem, &h->jvp_ctas, 0);
+    if (h->jvp_ctas < 1) h->jvp_ctas = 1;
+    h->jvp_small = h->small_mode != 0 && h->jvp_threads <= 256 && h->jvp_smem <= 56 * 1024 && bc_jvp_configure(S.dense, h->jvp_smem, 1) == cudaSuccess;
+    if (h->jvp_small) { bc_jvp_occupancy(S.dense, h->jvp_threads, h->jvp_smem, &h->jvp_ctas_small, 1); if (h->jvp_ctas_small <= h->jvp_ctas) h->jvp_small = 0; }
+    if (h->jvp_vec_global) h->jvp_ws_stride = bc_bwd_ws_doubles(n, m, npoly);
+  }
+  cudaGetLastError();   // (a refused configuration is not an error of this call)
   *out = h;
   return BCONE_OK;
 }
@@ -644,6 +664,40 @@ extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const do
   const int grid = std::min(B, h->num_sms * (use_small ? h->bwd_ctas_small : h->bwd_ctas));
   if (h->fast_bwd) CK(bc_bwdf_launch(&a, grid, h->bwd_threads, h->bwd_smem, st), "vjp launch (fast)");
   else CK(bc_bwd_launch(&a, grid, h->bwd_threads, h->bwd_smem, st, use_small), "vjp launch");
+  h->launches++;
+  return BCONE_OK;
+}
+
+extern "C" int bcone_jvp(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                         const double *x, const double *y, const double *s, const double *dA_vals, const double *dP_vals,
+                         const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters,
+                         const bcone_settings *stg, void *stream) {
+  Handle *h = (Handle *)handle;
+  if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !dA_vals || !db || !dc || !dx || !dy || !stg)
+    return fail(h, BCONE_EINVAL, "jvp: null argument");
+  if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "jvp: structure has P but P_vals is NULL");
+  if (!h->jvp_ok) return fail(h, BCONE_EUNSUPPORTED, "jvp: the instance does not fit the generic LSQR kernel");
+  cudaStream_t st = (cudaStream_t)stream;
+  BwdArgs a{};
+  a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
+  a.x = x; a.y = y; a.s = s;
+  a.tA = dA_vals; a.tP = h->S.nnzP > 0 ? dP_vals : nullptr; a.tb = db; a.tc = dc; a.tx = dx; a.ty = dy; a.ts = ds;
+  int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
+  a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
+  if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // no block-preconditioned forward mode
+  a.use_tma = h->tma_ok && (((uintptr_t)A_vals & 15) == 0); a.psd_total = h->psd_total; a.p_in_smem = h->jvp_p_in_smem;
+  CK(cudaSetDevice(h->device), "jvp set device");
+  a.ws_stride = (long long)h->jvp_ws_stride;
+  if (h->jvp_vec_global) {
+    Handle::StreamWs *sw = stream_ws(h, st);
+    if (!ensure_slab(h, &sw->jvp, nullptr, h->jvp_ws_stride * (size_t)h->num_sms * std::max(h->jvp_ctas, h->jvp_ctas_small))) return fail(h, BCONE_ENOMEM, "cudaMalloc jvp workspace");
+    a.ws = sw->jvp;
+  }
+  a.prof = h->prof;
+  CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "jvp counter");
+  const int use_small = h->jvp_small && (h->small_mode == 2 || B > h->num_sms * h->jvp_ctas);
+  const int grid = std::min(B, h->num_sms * (use_small ? h->jvp_ctas_small : h->jvp_ctas));
+  CK(bc_jvp_launch(&a, grid, h->jvp_threads, h->jvp_smem, st, use_small), "jvp launch");
   h->launches++;
   return BCONE_OK;
 }

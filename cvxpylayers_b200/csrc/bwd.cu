@@ -8,6 +8,7 @@
 //   dc = x r_tau - r_x;  dP_ij = (r_tau x_i - r_x,i) x_j (+ transpose term off the diagonal)
 // The instance's CSR values are staged once by TMA and stay in shared memory for all LSQR
 // iterations (each applies A and A' twice); P values are read from L2.
+// The same kernel with JVP = true is the forward-mode derivative (bcone_jvp), the transpose of the above.
 #include "common.cuh"
 
 struct BwdSmem {
@@ -251,7 +252,54 @@ __device__ void equilibrate(const BwdArgs &a, const BwdSmem &M, const double *Pg
   }
 }
 
-template <bool DENSE, bool SMALL = false>   // SMALL: <= 256 threads, four resident CTAs per SM (see fwd.cu)
+// U <- g = [-dA' pi_y - dc - dP x ; dA x - db ; pi_y'db + x'dc + x'dP x] for the data tangents of instance `inst`
+// (read from global memory; W holds dP x on the way).  Returns max|g| (block-uniform).  Starts with a barrier.
+// Not inlined: it runs once per instance, and inlined its products raise the spill of the LSQR loop.
+template <bool DENSE>
+__device__ __noinline__ double jvp_rhs(const BwdArgs &a, const BwdSmem &M, int inst, const ColPlan &plA, const ColPlan &plN) {
+  const DevStruct &S = a.S;
+  const int n = S.n, m = S.m, T = blockDim.x, t = threadIdx.x;
+  const double *tAg = a.tA + (size_t)inst * S.nnzA, *tbg = a.tb + (size_t)inst * m, *tcg = a.tc + (size_t)inst * n;
+  const double *tPg = (a.tP && S.nnzP > 0) ? a.tP + (size_t)inst * S.nnzP : nullptr;
+  for (int j = t; j < n; j += T) { M.U[j] = -tcg[j]; M.W[j] = 0.0; }
+  __syncthreads();
+  AT_mul<DENSE>(S, tAg, M.piy, M.part, [&](int j, double v) { M.U[j] -= v; }, plA);
+  if (tPg) P_mul(S, tPg, M.x, M.part, [&](int j, double v) { M.W[j] += v; }, plN);
+  A_mul<DENSE>(S, tAg, M.x, [&](int i, double v) { M.U[n + i] = v - tbg[i]; });
+  __syncthreads();
+  double d2[2] = {0, 0};
+  for (int j = t; j < n; j += T) {
+    const double w = M.W[j];
+    M.U[j] -= w; d2[0] = fma(M.x[j], w + tcg[j], d2[0]); d2[1] = fmax(d2[1], fabs(M.U[j]));
+  }
+  for (int i = t; i < m; i += T) { d2[0] = fma(M.piy[i], tbg[i], d2[0]); d2[1] = fmax(d2[1], fabs(M.U[n + i])); }
+  double s1[1] = {d2[0]}; block_reduce<1, false>(s1, M.red);
+  double m1[1] = {d2[1]}; block_reduce<1, true>(m1, M.red);
+  if (t == 0) M.U[n + m] = s1[0];
+  return fmax(m1[0], fabs(s1[0]));
+}
+
+// The equilibrated solve drops the unknown z_{n+i} of an inactive nonneg row together with its equation (row n+i of M is
+// [-A_i, e_i', b_i] and z_{n+i} appears nowhere else); dx and dy do not need it, ds does: recover it from that equation,
+// z_{n+i} = (dA x - db)_i + (A z_x)_i - b_i z_tau.  Ends with a barrier.
+template <bool DENSE>
+__device__ __noinline__ void jvp_inactive_rows(const BwdArgs &a, const BwdSmem &M, int inst) {
+  const DevStruct &S = a.S;
+  const int n = S.n, m = S.m, lo = S.z, hi = S.z + S.l;
+  const double *tAg = a.tA + (size_t)inst * S.nnzA, *tbg = a.tb + (size_t)inst * m;
+  const double zt = M.X[n + m];
+  auto inactive = [&](int i) { return i >= lo && i < hi && !(M.piy[i] > 0); };
+  A_mul<DENSE>(S, M.Av, M.X, [&](int i, double v) { if (inactive(i)) M.t1[i] = v - M.b[i] * zt; });
+  __syncthreads();
+  A_mul<DENSE>(S, tAg, M.x, [&](int i, double v) { if (inactive(i)) M.X[n + i] = M.t1[i] + v - tbg[i]; });
+  __syncthreads();
+}
+
+// JVP: the forward-mode derivative (bcone_jvp) instead of the adjoint -- the exact transpose of the map above:
+//   g  = [-dA' pi_y - dc - dP x ; dA x - db ; pi_y'db + x'dc + x'dP x]   (tangents dA, dP, db, dc read from global memory)
+//   z  = LSQR(M, g);  dx = z_x - x z_tau,  dy = D z_y - y z_tau,  ds = D z_y - z_y - s z_tau
+// The adjoint's gradient assembly is G' and its dz is E'w, so it computes G' M^-T E'w; this computes E M^-1 G.
+template <bool DENSE, bool SMALL = false, bool JVP = false>   // SMALL: <= 256 threads, four resident CTAs per SM (see fwd.cu)
 __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(const __grid_constant__ BwdArgs a) {
   extern __shared__ __align__(16) double smem[];
   const DevStruct &S = a.S;
@@ -295,7 +343,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
       if (i >= S.z + S.l) M.v[i] = vi;
       M.b[i] = a.b[(size_t)inst * m + i];
       M.piy[i] = (i >= S.z && i < S.z + S.l) ? fmax(vi, 0.0) : vi;
-      M.t1[i] = dyg[i];
+      if constexpr (!JVP) M.t1[i] = dyg[i];
     }
     if (a.use_tma) { mbar_wait(M.bar, tma_phase); tma_phase ^= 1; }
     __syncthreads();
@@ -350,19 +398,23 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
       xPx = d1[0];
     }
     for (int j = t; j < n; j += T) M.px2c[j] = 2.0 * M.px2c[j] + M.c[j];
-    // ---- dz -> U ----
-    apply_D(S, M, M.t1, M.t2);  // t2 = D dy   (also syncs px2c)
     double d3[3] = {0, 0, 0};
-    for (int j = t; j < n; j += T) { const double d = dxg[j]; M.U[j] = d; d3[0] = fma(M.x[j], d, d3[0]); d3[1] = fmax(d3[1], fabs(d)); }
-    for (int i = t; i < m; i += T) {
-      const double yi = a.y[(size_t)inst * m + i];
-      M.U[n + i] = M.t2[i]; d3[0] = fma(yi, M.t1[i], d3[0]); d3[1] = fmax(d3[1], fabs(M.t2[i]));
-    }
-    {
-      double s1[1] = {d3[0]}; block_reduce<1, false>(s1, M.red);
-      double m1[1] = {d3[1]}; block_reduce<1, true>(m1, M.red);
-      if (t == 0) M.U[N - 1] = -s1[0];
-      d3[1] = fmax(m1[0], fabs(s1[0]));
+    if constexpr (JVP) {
+      d3[1] = jvp_rhs<DENSE>(a, M, inst, plA, plN);   // g -> U (syncs px2c)
+    } else {
+      // ---- dz -> U ----
+      apply_D(S, M, M.t1, M.t2);  // t2 = D dy   (also syncs px2c)
+      for (int j = t; j < n; j += T) { const double d = dxg[j]; M.U[j] = d; d3[0] = fma(M.x[j], d, d3[0]); d3[1] = fmax(d3[1], fabs(d)); }
+      for (int i = t; i < m; i += T) {
+        const double yi = a.y[(size_t)inst * m + i];
+        M.U[n + i] = M.t2[i]; d3[0] = fma(yi, M.t1[i], d3[0]); d3[1] = fmax(d3[1], fabs(M.t2[i]));
+      }
+      {
+        double s1[1] = {d3[0]}; block_reduce<1, false>(s1, M.red);
+        double m1[1] = {d3[1]}; block_reduce<1, true>(m1, M.red);
+        if (t == 0) M.U[N - 1] = -s1[0];
+        d3[1] = fmax(m1[0], fabs(s1[0]));
+      }
     }
     __syncthreads();
     int itn = 0;
@@ -374,23 +426,29 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
       const double ctol = st.lsqr_conlim > 0 ? 1.0 / st.lsqr_conlim : 0.0;
       const int iter_lim = st.lsqr_iter_lim < 0 ? 2 * N : st.lsqr_iter_lim;
       const bool pc = st.lsqr_precond != 0;
+      // row / column scaling of B: the equilibration is computed for M', so M takes it with the two sides swapped
+      // (an inactive nonneg row zeroes column n+i of M, which is e_{n+i}, and row n+i: see jvp_inactive_rows)
+      double *const Ls = JVP ? M.Rsc : M.Lsc, *const Rs = JVP ? M.Lsc : M.Rsc;
       if (pc) {
         equilibrate<DENSE>(a, M, Pg, xPx, st.ruiz_passes > 0 ? st.ruiz_passes : 10, plA, plN);
-        for (int k = t; k < N; k += T) { M.U[k] *= M.Lsc[k]; M.X[k] = 0.0; }
+        for (int k = t; k < N; k += T) { M.U[k] *= Ls[k]; M.X[k] = 0.0; }
         __syncthreads();
       }
-      // B = diag(Lsc) M' diag(Rsc)  (identity scalings when lsqr_precond = 0); both products accumulate
+      // B = diag(Lsc) M' diag(Rsc), or diag(Rsc) M diag(Lsc) for the JVP  (identity scalings when lsqr_precond = 0);
+      // both products accumulate
       auto acc_B = [&](const double *in, double *out) {   // out += B in
         const double *src = in;
-        if (pc) { for (int k = t; k < N; k += T) M.tin[k] = M.Rsc[k] * in[k]; src = M.tin; }
+        if (pc) { for (int k = t; k < N; k += T) M.tin[k] = Rs[k] * in[k]; src = M.tin; }
         __syncthreads();
-        op_MT<DENSE>(a, M, Pg, xPx, src, out, pc ? M.Lsc : nullptr, plA, plN);
+        if constexpr (JVP) op_M<DENSE>(a, M, Pg, xPx, src, out, pc ? Ls : nullptr, plA, plN);
+        else op_MT<DENSE>(a, M, Pg, xPx, src, out, pc ? Ls : nullptr, plA, plN);
       };
       auto acc_BT = [&](const double *in, double *out) {  // out += B' in
         const double *src = in;
-        if (pc) { for (int k = t; k < N; k += T) M.tin[k] = M.Lsc[k] * in[k]; src = M.tin; }
+        if (pc) { for (int k = t; k < N; k += T) M.tin[k] = Ls[k] * in[k]; src = M.tin; }
         __syncthreads();
-        op_M<DENSE>(a, M, Pg, xPx, src, out, pc ? M.Rsc : nullptr, plA, plN);
+        if constexpr (JVP) op_MT<DENSE>(a, M, Pg, xPx, src, out, pc ? Rs : nullptr, plA, plN);
+        else op_M<DENSE>(a, M, Pg, xPx, src, out, pc ? Rs : nullptr, plA, plN);
       };
       double r1[1] = {0};
       for (int k = t; k < N; k += T) r1[0] = fma(M.U[k], M.U[k], r1[0]);
@@ -460,9 +518,21 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
           if (istop) break;
         }
       }
-      if (pc) { __syncthreads(); for (int k = t; k < N; k += T) M.X[k] *= M.Rsc[k]; }
+      if (pc) { __syncthreads(); for (int k = t; k < N; k += T) M.X[k] *= Rs[k]; }
+      if constexpr (JVP) if (pc && S.l > 0) { __syncthreads(); jvp_inactive_rows<DENSE>(a, M, inst); }
     }
     __syncthreads();
+    if constexpr (JVP) {   // ---- solution tangents: dx = z_x - x z_tau, dy = D z_y - y z_tau, ds = D z_y - z_y - s z_tau ----
+      apply_D(S, M, M.X + n, M.t2);
+      const double zt = M.X[N - 1];
+      for (int j = t; j < n; j += T) a.tx[(size_t)inst * n + j] = M.X[j] - M.x[j] * zt;
+      for (int i = t; i < m; i += T) {
+        const size_t k = (size_t)inst * m + i;
+        a.ty[k] = M.t2[i] - a.y[k] * zt;
+        if (a.ts) a.ts[k] = M.t2[i] - M.X[n + i] - a.s[k] * zt;
+      }
+      if (t == 0 && a.lsqr_iters) a.lsqr_iters[inst] = itn;
+    } else
     // ---- gradient assembly (every structural entry; SURVEY.md 8a B4 + the A.nonzero() hazard) ----
     {
       const double rt = M.X[N - 1];
@@ -513,5 +583,26 @@ extern "C" cudaError_t bc_bwd_occupancy(int dense, int threads, size_t smem, int
 extern "C" cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta) {
   const int dense = a->S.dense;
   BWD_DISPATCH((k<<<grid, threads, smem, stream>>>(*a)));
+  return cudaGetLastError();
+}
+// forward-mode derivative: same kernel, same shared-memory layout, JVP = true
+#define JVP_DISPATCH(EXPR)                                                     \
+  do {                                                                         \
+    if (small_cta) { if (dense) { auto k = bwd_kernel<true, true, true>; EXPR; } else { auto k = bwd_kernel<false, true, true>; EXPR; } } \
+    else { if (dense) { auto k = bwd_kernel<true, false, true>; EXPR; } else { auto k = bwd_kernel<false, false, true>; EXPR; } }         \
+  } while (0)
+extern "C" cudaError_t bc_jvp_configure(int dense, size_t smem, int small_cta) {
+  cudaError_t e = cudaSuccess;
+  JVP_DISPATCH(e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  return e;
+}
+extern "C" cudaError_t bc_jvp_occupancy(int dense, int threads, size_t smem, int *ctas_per_sm, int small_cta) {
+  cudaError_t e = cudaSuccess;
+  JVP_DISPATCH(e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, threads, smem));
+  return e;
+}
+extern "C" cudaError_t bc_jvp_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta) {
+  const int dense = a->S.dense;
+  JVP_DISPATCH((k<<<grid, threads, smem, stream>>>(*a)));
   return cudaGetLastError();
 }

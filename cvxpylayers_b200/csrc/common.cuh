@@ -79,6 +79,10 @@ struct BwdArgs {
   unsigned long long *prof;     // optional: [16] phase cycle counters (debug, bcone_set_profile)
   double *ws;            // large instances: LSQR vectors live in a per-CTA slab of global memory (L2)
   long long ws_stride;
+  // forward-mode derivative (bcone_jvp, bwd_kernel<.., .., true>): tangents of the data in (tP may be NULL = 0),
+  // tangents of the solution out (ts may be NULL).  Unused by the adjoint kernels.
+  const double *tA, *tP, *tb, *tc;
+  double *tx, *ty, *ts;
 };
 
 // Phase timing (debug): thread 0 of every CTA adds the cycles since the previous stamp to prof[phase].

@@ -352,3 +352,32 @@ class Engine:
                                 _ptr(its), C.byref(settings), self._stream())
         self._raise(rc, "bcone_vjp")
         return dA, dP, db, dc, its
+
+    def jvp(self, A_vals, b, c, x, y, s, dA, db, dc, P_vals=None, dP=None, settings: _lib.BconeSettings | None = None, out=None):
+        """Forward-mode derivative of the solution map at (x, y, s) (diffcp's ``D``; the transpose of :meth:`vjp`): tangents of
+        the data in engine layout -> dx[B,n], dy[B,m], ds[B,m], lsqr_iters[B]  (``out``: the same four, preallocated).
+        ``dP`` None = no tangent on P."""
+        st, dev, f64 = self.structure, self.device, torch.float64
+        B = A_vals.shape[0]
+        for name, t, shp in (("A_vals", A_vals, (B, st.nnzA)), ("b", b, (B, st.m)), ("c", c, (B, st.n)),
+                             ("x", x, (B, st.n)), ("y", y, (B, st.m)), ("s", s, (B, st.m)),
+                             ("dA", dA, (B, st.nnzA)), ("db", db, (B, st.m)), ("dc", dc, (B, st.n))):
+            _chk(t, shp, f64, dev, name)
+        if st.nnzP:
+            if P_vals is None:
+                raise ValueError("structure has a quadratic term but P_vals is None")
+            _chk(P_vals, (B, st.nnzP), f64, dev, "P_vals")
+            _chk(dP, (B, st.nnzP), f64, dev, "dP")
+        settings = settings or _lib.default_settings()
+        if out is not None:
+            dx, dy, ds, its = out
+        else:
+            dx = torch.empty((B, st.n), dtype=f64, device=dev)
+            dy = torch.empty((B, st.m), dtype=f64, device=dev)
+            ds = torch.empty((B, st.m), dtype=f64, device=dev)
+            its = torch.empty(B, dtype=torch.int32, device=dev)
+        rc = self.lib.bcone_jvp(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c),
+                                _ptr(x), _ptr(y), _ptr(s), _ptr(dA), _ptr(dP if st.nnzP else None), _ptr(db), _ptr(dc),
+                                _ptr(dx), _ptr(dy), _ptr(ds), _ptr(its), C.byref(settings), self._stream())
+        self._raise(rc, "bcone_jvp")
+        return dx, dy, ds, its

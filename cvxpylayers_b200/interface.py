@@ -198,6 +198,21 @@ class _Saved:
         self.items = items
 
 
+def _forward_ad_active() -> bool:
+    """Inside ``torch.autograd.forward_ad.dual_level()``: a Function's ``jvp`` may run for dual inputs that do not require
+    grad, so what it needs is kept whatever ``needs_grad`` says (the reference computes that from ``requires_grad`` only)."""
+    from torch.autograd import forward_ad  # noqa: PLC0415
+
+    return forward_ad._current_level >= 0
+
+
+def _tangent(t: torch.Tensor | None, rows: int, B: int, unbatched: bool, dev: torch.device) -> torch.Tensor:
+    """A boundary-layout input tangent [rows, B] on the engine's device; None (no tangent) is zero."""
+    if t is None:
+        return torch.zeros((rows, B), dtype=torch.float64, device=dev)
+    return _to_dev(t.unsqueeze(1) if unbatched else t, dev)
+
+
 def _to_dev(t: torch.Tensor | None, dev: torch.device) -> torch.Tensor | None:
     """Host -> device (asynchronous DMA when the caller's tensor is pinned)."""
     if t is None:
@@ -466,7 +481,8 @@ class _CvxpyLayer(torch.autograd.Function):
                 dual = _to_host_like(sol.y, in_device, in_dtype)
                 if in_device.type == "cpu":
                     torch.cuda.current_stream(dev).synchronize()
-        saved = _Saved(eng, settings, A_vals, P_vals, b, c, sol.x, sol.y, sol.s, piped, A_eval.shape[0]) if needs_grad else None
+        keep = needs_grad or _forward_ad_active()
+        saved = _Saved(eng, settings, A_vals, P_vals, b, c, sol.x, sol.y, sol.s, piped, A_eval.shape[0]) if keep else None
         return primal, dual, saved, (batch_size, originally_unbatched, in_device, in_dtype, use_P)
 
     @staticmethod
@@ -508,6 +524,27 @@ class _CvxpyLayer(torch.autograd.Function):
             dA_eval = dA_eval.squeeze(1)
             dP_eval = dP_eval.squeeze(1) if dP_eval is not None else None
         return dP_eval, dq_eval, dA_eval, None, None, None, None
+
+    @staticmethod
+    def jvp(ctx: Any, tP, tq, tA, *_):
+        """Forward mode (diffcp's ``D``): the boundary tangents go through the same ingest maps as the data (they are linear),
+        then ``bcone_jvp``.  Tangents come back where the outputs live; absent ones are zero."""
+        batch_size, originally_unbatched, in_device, in_dtype, use_P = ctx.backward_data
+        if ctx.saved is None:
+            raise RuntimeError("forward-mode AD on a forward pass that kept nothing for it")
+        eng, settings, A_vals, P_vals, b, c, x, y, s, _piped, nnz_aug = ctx.saved.items
+        dev = eng.device
+        with torch.cuda.device(dev):
+            tA_e = _tangent(tA, nnz_aug, batch_size, originally_unbatched, dev)
+            tq_e = _tangent(tq, eng.structure.n + 1, batch_size, originally_unbatched, dev)
+            tP_e = _tangent(tP, eng._nnzP_b, batch_size, originally_unbatched, dev) if (use_P and tP is not None) else None
+            dA, dP, db, dc = eng.ingest(tA_e, tq_e, tP_e)
+            dx, dy, _, _ = eng.jvp(A_vals, b, c, x, y, s, dA, db, dc, P_vals, dP, settings)
+            dprimal = _to_host_like(dx, in_device, in_dtype)
+            ddual = _to_host_like(dy, in_device, in_dtype)
+            if in_device.type == "cpu":
+                torch.cuda.current_stream(dev).synchronize()
+        return dprimal, ddual, None, None
 
 
 def get_solver_ctx(solver, param_prob, cone_dims, data, kwargs, verbose=False):
@@ -574,7 +611,7 @@ class _CvxpyLayerFused(torch.autograd.Function):
             dual = _to_host_like(sol.y, in_device, in_dtype)
             if in_device.type == "cpu":
                 torch.cuda.current_stream(dev).synchronize()
-        saved = _Saved(eng, settings, A_vals, P_vals, b, c, sol.x, sol.y, sol.s) if needs_grad else None
+        saved = _Saved(eng, settings, A_vals, P_vals, b, c, sol.x, sol.y, sol.s) if (needs_grad or _forward_ad_active()) else None
         return primal, dual, saved, (unb, in_device, in_dtype)
 
     @staticmethod
@@ -596,6 +633,24 @@ class _CvxpyLayerFused(torch.autograd.Function):
             if in_device.type == "cpu":
                 torch.cuda.current_stream(dev).synchronize()
         return (dp.squeeze(1) if unb else dp), None, None, None, None
+
+    @staticmethod
+    def jvp(ctx: Any, tp, *_):
+        """Forward mode: the tangent of ``p_stack`` through the parameter maps (linear in ``p_stack``), then ``bcone_jvp``."""
+        unb, in_device, in_dtype = ctx.backward_data
+        if ctx.saved is None:
+            raise RuntimeError("forward-mode AD on a forward pass that kept nothing for it")
+        eng, settings, A_vals, P_vals, b, c, x, y, s = ctx.saved.items
+        dev = eng.device
+        B = A_vals.shape[0]
+        with torch.cuda.device(dev):
+            dA, dP, db, dc = eng.ingest_params(_tangent(tp, eng._P1, B, unb, dev))
+            dx, dy, _, _ = eng.jvp(A_vals, b, c, x, y, s, dA, db, dc, P_vals, dP, settings)
+            dprimal = _to_host_like(dx, in_device, in_dtype)
+            ddual = _to_host_like(dy, in_device, in_dtype)
+            if in_device.type == "cpu":
+                torch.cuda.current_stream(dev).synchronize()
+        return dprimal, ddual, None, None
 
 
 _REGISTERED = False

@@ -97,6 +97,24 @@ class _FlattenParams(torch.autograd.Function):
             outs.append(gp)
         return (None, None, *outs)
 
+    @staticmethod
+    def jvp(ctx: Any, _spec, _B, *tangents):
+        """Forward mode: the same index maps on the tangents (d log p = dp / p for GP-log parameters); the constant row's
+        tangent is 0, as is the rows' of a parameter without one."""
+        lib = _lib.load()
+        dev = ctx.keep[0].device
+        P1 = sum(s[1] for s in ctx.spec) + 1
+        tp = torch.zeros((P1, ctx.B), dtype=torch.float64, device=dev)
+        for (row0, size, batched, shape, op), pc, t in zip(ctx.spec, ctx.keep, tangents):
+            if t is None:
+                continue
+            tc = t.detach().to(dtype=torch.float64)
+            tc = (tc / pc if op == OP_LOG else tc).contiguous()
+            fmap = _dev_i32(("F", shape), lambda shape=shape: fortran_map(shape), dev)
+            _chk(lib.bcone_rows_from_param(_p(tc), C.c_int64(size if batched else 0), _p(fmap), C.c_int32(size), C.c_int32(ctx.B), C.c_int32(OP_NONE),
+                                           C.c_void_p(tp.data_ptr() + row0 * ctx.B * 8), _stream(dev)), "bcone_rows_from_param")
+        return tp
+
 
 def flatten_and_batch_params(params: tuple[torch.Tensor, ...], ctx, batch: tuple) -> torch.Tensor:
     """Device twin of ``_flatten_and_batch_params(params, ctx, batch)`` (+ the GP log of ``_apply_gp_log_transform``,
@@ -144,6 +162,21 @@ class _GatherCols(torch.autograd.Function):
         _chk(lib.bcone_scatter_cols(_p(g), _p(out), C.c_int64(ld), _p(imap), _p(scale), C.c_int32(K), C.c_int32(B), C.c_int32(op), _p(gin),
                                     _stream(g.device)), "bcone_scatter_cols")
         return gin, None, None, None
+
+    @staticmethod
+    def jvp(ctx: Any, tsrc, *_):
+        """Forward mode: the same gather on the tangent (times ``out`` for GP-exp variables: d exp(u) = exp(u) du)."""
+        lib = _lib.load()
+        imap, scale, op, ld, out = ctx.meta
+        K = imap.numel()
+        if tsrc is None:
+            return None
+        ts = tsrc.detach().contiguous()
+        B = ts.shape[0]
+        tout = torch.empty((B, K), dtype=torch.float64, device=ts.device)
+        _chk(lib.bcone_gather_cols(_p(ts), C.c_int64(ld), _p(imap), _p(scale), C.c_int32(K), C.c_int32(B), C.c_int32(OP_NONE), _p(tout),
+                                   _stream(ts.device)), "bcone_gather_cols")
+        return tout * out if op == OP_EXP else tout
 
 
 def _var_map(var) -> tuple[np.ndarray, np.ndarray | None]:

@@ -14,6 +14,7 @@
  *   bcone_solve    <- diffcp.solve_and_derivative_batch / solve_only_batch
  *                                                    diffcp_if.py:365, :369 (SCS forward solve)
  *   bcone_vjp      <- the adjoint closure adj_batch  diffcp_if.py:86      (diffcp adjoint_derivative)
+ *   bcone_jvp      <- diffcp's forward derivative D  (second output of solve_and_derivative; the reference never calls it)
  *   bcone_emit     <- _compute_gradients re-packing  diffcp_if.py:88-94 + stacks :396-397
  *                     (dA_eval = [-dA ; db[b_idx]], dq_eval = [dc ; 0])
  *
@@ -171,6 +172,18 @@ int bcone_vjp(void *handle, int32_t B, const double *A_vals, const double *P_val
               const double *c, const double *x, const double *y, const double *s, const double *dx,
               const double *dy, double *dA_vals, double *dP_vals, double *db, double *dc,
               int32_t *lsqr_iters, const bcone_settings *st, void *cuda_stream);
+
+/* Forward mode (stateless): derivative of the solution map at (x,y,s) applied to tangents of the data -- diffcp's
+ * solve_and_derivative `D` (the reference's backend returns it next to the adjoint `DT` that bcone_vjp provides).  Exactly the
+ * transpose of bcone_vjp: <(dx,dy), bcone_jvp(dA,dP,db,dc)> = <bcone_vjp(dx,dy), (dA,dP,db,dc)>.  Tangents in engine layout:
+ * dA_vals[B,nnzA], dP_vals[B,nnzP] (upper-triangular values, an off-diagonal one perturbs P_ij and P_ji) or NULL = 0, db[B,m],
+ * dc[B,n].  Outputs dx[B,n], dy[B,m], ds[B,m] or NULL, lsqr_iters[B] or NULL (0 where the tangent is zero).  Boundary-layout
+ * tangents go through bcone_ingest / bcone_ingest_params first (both are linear; a tangent's constant row is 0).  Always the
+ * generic LSQR kernel; lsqr_precond = 2 runs as 1.  BCONE_EUNSUPPORTED when the instance does not fit that kernel. */
+int bcone_jvp(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+              const double *x, const double *y, const double *s, const double *dA_vals, const double *dP_vals,
+              const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters,
+              const bcone_settings *st, void *cuda_stream);
 
 /* Pitched host<->device copy on the caller's stream (bytes): moves a batch slice [rows, lo:hi] of a
  * boundary tensor directly between pinned host memory and a contiguous device chunk. */
