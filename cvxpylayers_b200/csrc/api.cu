@@ -12,11 +12,11 @@
 
 // ---- kernels / launchers implemented in fwd.cu, bwd.cu, pack.cu ----
 extern "C" {
-size_t bc_fwd_smem_bytes(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp);
-size_t bc_fwd_ws_doubles(int n, int m, int with_factor);
-cudaError_t bc_fwd_configure(int dense, int indirect, size_t smem, int small_cta);
-cudaError_t bc_fwd_occupancy(int dense, int indirect, int threads, size_t smem, int *ctas, int small_cta);
-cudaError_t bc_fwd_launch(const FwdArgs *a, int indirect, int grid, int threads, size_t smem, cudaStream_t st, int small_cta);
+size_t bc_fwd_smem_bytes(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp, int vals_global);
+size_t bc_fwd_ws_doubles(int n, int m, int vectors, int with_factor, int nnzA_global);
+cudaError_t bc_fwd_configure(int dense, int indirect, size_t smem, int small_cta, int vg);
+cudaError_t bc_fwd_occupancy(int dense, int indirect, int threads, size_t smem, int *ctas, int small_cta, int vg);
+cudaError_t bc_fwd_launch(const FwdArgs *a, int indirect, int grid, int threads, size_t smem, cudaStream_t st, int small_cta, int vg);
 size_t bc_fwdf_smem_bytes(int n, int m);
 int bc_fwdf_threads(void);
 size_t bc_fwdf_cache_doubles(int n, int m);
@@ -25,13 +25,13 @@ cudaError_t bc_fwdf_configure(int n, int m, size_t smem);
 cudaError_t bc_fwdf_occupancy(int n, int m, size_t smem, int *ctas);
 cudaError_t bc_fwdf_launch(const FwdArgs *a, int grid, size_t smem, cudaStream_t st);
 size_t bc_bwd_ws_doubles(int n, int m, int npoly);
-size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global);
-cudaError_t bc_bwd_configure(int dense, size_t smem, int small_cta);
-cudaError_t bc_bwd_occupancy(int dense, int threads, size_t smem, int *ctas, int small_cta);
-cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st, int small_cta);
-cudaError_t bc_jvp_configure(int dense, size_t smem, int small_cta);
-cudaError_t bc_jvp_occupancy(int dense, int threads, size_t smem, int *ctas, int small_cta);
-cudaError_t bc_jvp_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st, int small_cta);
+size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global, int vals_global);
+cudaError_t bc_bwd_configure(int dense, size_t smem, int small_cta, int vg);
+cudaError_t bc_bwd_occupancy(int dense, int threads, size_t smem, int *ctas, int small_cta, int vg);
+cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st, int small_cta, int vg);
+cudaError_t bc_jvp_configure(int dense, size_t smem, int small_cta, int vg);
+cudaError_t bc_jvp_occupancy(int dense, int threads, size_t smem, int *ctas, int small_cta, int vg);
+cudaError_t bc_jvp_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st, int small_cta, int vg);
 size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads);
 cudaError_t bc_bwdf_configure(int n, size_t smem);
 cudaError_t bc_bwdf_occupancy(int n, int threads, size_t smem, int *ctas);
@@ -88,6 +88,9 @@ struct Handle {
   // forward-mode derivative (bcone_jvp): always the generic kernel (bwd.cu, JVP = true), so structures on the fused backward
   // need a generic geometry of their own; chosen by the same rule as the generic backward's.  jvp_ok = 0: none fits.
   int jvp_ok = 0, jvp_threads = 0, jvp_p_in_smem = 0, jvp_vec_global = 0, jvp_ctas = 0, jvp_small = 0, jvp_ctas_small = 0;
+  // values off chip (the tier after every on-chip option): the forward copies each instance's CSR values into its CTA's slab,
+  // the backward / forward-mode LSQR reads them in place from A_vals.  Only 512-thread builds exist for it (no SMALL variant).
+  int fwd_vals_global = 0, bwd_vals_global = 0, jvp_vals_global = 0;
   size_t jvp_smem = 0, jvp_ws_stride = 0;
   long long launches = 0;
   int last_block_slot = -1;   // ring slot of the last block-preconditioned vjp (its fallback counter is read by bcone_fallback_count)
@@ -122,7 +125,7 @@ Handle::StreamWs *stream_ws(Handle *h, cudaStream_t s) {
 bool ensure_slab(Handle *h, double **p, size_t *cap, size_t doubles) {
   if (*p && (!cap || *cap >= doubles)) return true;
   double *q = nullptr;
-  if (cudaMalloc((void **)&q, doubles * sizeof(double)) != cudaSuccess) return false;
+  if (cudaMalloc((void **)&q, doubles * sizeof(double)) != cudaSuccess) { cudaGetLastError(); return false; }   // (not left for the next launch check)
   h->allocs.push_back(q);   // (an outgrown slab stays alive until destroy: a kernel in flight may still use it)
   *p = q;
   if (cap) *cap = doubles;
@@ -231,33 +234,40 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
   // per CTA); else INDIRECT (conjugate gradients, SCS's "indirect" mode).  BCONE_FWD_MODE=indirect forces the last one.
   const char *fm = getenv("BCONE_FWD_MODE");
   const bool force_indirect = fm && std::string(fm) == "indirect";
+  // Last tier, for instances whose CSR values do not fit next to the rest: the values in global memory (L2 when the grid's
+  // working set fits, HBM otherwise), the same rule for everything else.  Tried only after every on-chip option has failed;
+  // BCONE_VALUES_GLOBAL=1 selects it for every generic kernel of a structure that would fit on chip (a test hook).
+  const char *vgv = getenv("BCONE_VALUES_GLOBAL");
+  const int vals_lo = (vgv && atoi(vgv)) ? 1 : 0;
   auto pick_fwd = [&]() -> bool {
-    for (int ind = 0; ind <= 1; ind++)
-      for (int tt = threads; tt >= 64; tt /= 2) {
-        size_t sm = bc_fwd_smem_bytes(n, m, d->nnzA, tt, max_psd, ind, d->ns, d->ep + d->ed);
-        if (sm <= smem_cap) {
-          h->fwd_threads = tt; h->fwd_smem = sm; h->fwd_indirect = ind;
-          // (n <= 512: one thread per column in the transposed triangular product; on the sparse LP with n = 1000 the slab mode
-          //  streams 8 MB of factor per iteration and CTA from HBM and loses to conjugate gradients, while at n = 101 the factor
-          //  stays in L2 and the slab mode wins by a wide margin)
-          if (ind && !force_indirect && n <= 512) { h->fwd_indirect = 0; h->fwd_factor_global = 1; }
-          return true;
-        }
-      }
-    return false;
-  };
-  // generic LSQR kernel (bwd.cu): prefer P staged in shared memory, then vectors on chip, then vectors in L2
-  auto pick_generic = [&](int &g_threads, size_t &g_smem, int &g_p_in_smem, int &g_vec_global) -> bool {
-    for (int vg = 0; vg <= 1; vg++)
-      for (int psm = (S.nnzP > 0 ? 1 : 0); psm >= 0; psm--)
+    for (int vals = vals_lo; vals <= 1; vals++)
+      for (int ind = 0; ind <= 1; ind++)
         for (int tt = threads; tt >= 64; tt /= 2) {
-          size_t sm = bc_bwd_smem_bytes(n, m, npoly, d->nnzA, psm ? S.nnzP : 0, tt, max_psd, psd_total, d->ep + d->ed, vg);
-          if (sm <= smem_cap) { g_threads = tt; g_smem = sm; g_p_in_smem = psm; g_vec_global = vg; return true; }
-          if (psm) break;  // do not trade threads for P residency
+          size_t sm = bc_fwd_smem_bytes(n, m, d->nnzA, tt, max_psd, ind, d->ns, d->ep + d->ed, vals);
+          if (sm <= smem_cap) {
+            h->fwd_threads = tt; h->fwd_smem = sm; h->fwd_indirect = ind; h->fwd_vals_global = vals;
+            // (n <= 512: one thread per column in the transposed triangular product; on the sparse LP with n = 1000 the slab mode
+            //  streams 8 MB of factor per iteration and CTA from HBM and loses to conjugate gradients, while at n = 101 the factor
+            //  stays in L2 and the slab mode wins by a wide margin)
+            if (ind && !force_indirect && n <= 512) { h->fwd_indirect = 0; h->fwd_factor_global = 1; }
+            return true;
+          }
         }
     return false;
   };
-  auto pick_bwd = [&]() -> bool { return pick_generic(h->bwd_threads, h->bwd_smem, h->p_in_smem, h->bwd_vec_global); };
+  // generic LSQR kernel (bwd.cu): prefer P staged in shared memory, then vectors on chip, then vectors in L2; values off chip last
+  auto pick_generic = [&](int &g_threads, size_t &g_smem, int &g_p_in_smem, int &g_vec_global, int &g_vals_global) -> bool {
+    for (int vals = vals_lo; vals <= 1; vals++)
+      for (int vg = 0; vg <= 1; vg++)
+        for (int psm = (S.nnzP > 0 ? 1 : 0); psm >= 0; psm--)
+          for (int tt = threads; tt >= 64; tt /= 2) {
+            size_t sm = bc_bwd_smem_bytes(n, m, npoly, d->nnzA, psm ? S.nnzP : 0, tt, max_psd, psd_total, d->ep + d->ed, vg, vals);
+            if (sm <= smem_cap) { g_threads = tt; g_smem = sm; g_p_in_smem = psm; g_vec_global = vg; g_vals_global = vals; return true; }
+            if (psm) break;  // do not trade threads for P residency
+          }
+    return false;
+  };
+  auto pick_bwd = [&]() -> bool { return pick_generic(h->bwd_threads, h->bwd_smem, h->p_in_smem, h->bwd_vec_global, h->bwd_vals_global); };
   // fast backward path: same launch geometry fields, different kernel
   if (S.dense && S.ncones == 0 && d->ep + d->ed == 0 && n <= 128 && (n % 2) == 0 && (S.nnzP == 0 || S.p_dense)) {
     for (int tt = threads; tt >= 64; tt /= 2) {
@@ -272,9 +282,27 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
     }
   }
   if (!pick_fwd() || (!h->fast_bwd && !pick_bwd())) {
-    char buf[256];
-    snprintf(buf, sizeof buf, "instance does not fit the shared-memory-resident engine (fwd %zu B / bwd %zu B needed, %zu B per CTA available)",
-             bc_fwd_smem_bytes(n, m, d->nnzA, 64, max_psd, 1, d->ns, d->ep + d->ed), bc_bwd_smem_bytes(n, m, npoly, d->nnzA, 0, 64, max_psd, psd_total, d->ep + d->ed, 1), smem_cap);
+    // With values and vectors off chip, what is left in shared memory is the per-CTA scratch: the cone scratch (per-warp PSD
+    // scratch, persistent eigenvectors, exp-cone slots) and the 8 n column partials.  Name the largest PSD order that would fit.
+    auto need = [&](int k, size_t *f, size_t *b) {
+      int pt = 0;
+      for (int i = 0; i < d->ns; i++) { const int kk = std::min(d->s[i], k); pt += kk * kk + kk; }
+      *f = bc_fwd_smem_bytes(n, m, d->nnzA, 64, k, 1, k > 0 ? d->ns : 0, d->ep + d->ed, 1);
+      *b = bc_bwd_smem_bytes(n, m, npoly, d->nnzA, 0, 64, k, pt, d->ep + d->ed, 1, 1);
+      return *f <= smem_cap && *b <= smem_cap;
+    };
+    size_t fb = 0, bb = 0, f2 = 0, b2 = 0;
+    need(max_psd, &fb, &bb);
+    int kfit = -1;
+    for (int k = max_psd; k >= 0 && kfit < 0; k--) if (need(k, &f2, &b2)) kfit = k;
+    char buf[512];
+    if (max_psd > 0 && kfit >= 0)
+      snprintf(buf, sizeof buf, "instance does not fit the engine: even with the CSR values and the vectors in global memory, the on-chip cone scratch "
+               "(per-warp PSD scratch and persistent eigenvectors of PSD order %d) needs fwd %zu B / bwd %zu B, %zu B per CTA available; "
+               "the largest PSD order that fits is %d", max_psd, fb, bb, smem_cap, kfit);
+    else
+      snprintf(buf, sizeof buf, "instance does not fit the engine: even with the CSR values and the vectors in global memory, the on-chip scratch "
+               "(cone scratch and 8 n = %d column partials) needs fwd %zu B / bwd %zu B, %zu B per CTA available", 8 * n, fb, bb, smem_cap);
     bcone_destroy(h);
     return fail(nullptr, BCONE_EUNSUPPORTED, buf);
   }
@@ -290,37 +318,40 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
     const char *sc = getenv("BCONE_SMALL_CTA");
     h->small_mode = sc ? atoi(sc) : 1;
     const bool allow = h->small_mode != 0;
-    h->fwd_small = allow && !h->fast_fwd && !h->fwd_indirect && h->fwd_threads <= 256 && h->fwd_smem <= 56 * 1024;
-    h->bwd_small = allow && !h->fast_bwd && h->bwd_threads <= 256 && h->bwd_smem <= 56 * 1024;
+    h->fwd_small = allow && !h->fast_fwd && !h->fwd_indirect && !h->fwd_vals_global && h->fwd_threads <= 256 && h->fwd_smem <= 56 * 1024;
+    h->bwd_small = allow && !h->fast_bwd && !h->bwd_vals_global && h->bwd_threads <= 256 && h->bwd_smem <= 56 * 1024;
   }
-  if (h->fwd_small && bc_fwd_configure(S.dense, 0, h->fwd_smem, 1) != cudaSuccess) h->fwd_small = 0;
-  if (h->bwd_small && bc_bwd_configure(S.dense, h->bwd_smem, 1) != cudaSuccess) h->bwd_small = 0;
-  if ((e = bc_fwd_configure(S.dense, h->fwd_indirect, h->fast_fwd ? bc_fwd_smem_bytes(n, m, d->nnzA, 64, max_psd, h->fwd_indirect, d->ns, d->ep + d->ed) : h->fwd_smem, 0)) != cudaSuccess ||
-      (e = (h->fast_bwd ? bc_bwdf_configure(n, h->bwd_smem) : bc_bwd_configure(S.dense, h->bwd_smem, 0))) != cudaSuccess) {
+  const int fvg = h->fwd_vals_global, bvg = h->bwd_vals_global;
+  if (h->fwd_small && bc_fwd_configure(S.dense, 0, h->fwd_smem, 1, 0) != cudaSuccess) h->fwd_small = 0;
+  if (h->bwd_small && bc_bwd_configure(S.dense, h->bwd_smem, 1, 0) != cudaSuccess) h->bwd_small = 0;
+  if ((e = bc_fwd_configure(S.dense, h->fwd_indirect, h->fast_fwd ? bc_fwd_smem_bytes(n, m, d->nnzA, 64, max_psd, h->fwd_indirect, d->ns, d->ep + d->ed, fvg) : h->fwd_smem, 0, fvg)) != cudaSuccess ||
+      (e = (h->fast_bwd ? bc_bwdf_configure(n, h->bwd_smem) : bc_bwd_configure(S.dense, h->bwd_smem, 0, bvg))) != cudaSuccess) {
     std::string msg = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e);
     bcone_destroy(h);
     return fail(nullptr, BCONE_ECUDA, msg);
   }
   if (h->block_bwd && (e = bc_bwdb_configure(h->blk_smem)) != cudaSuccess) h->block_bwd = 0;
   if (h->fast_fwd) bc_fwdf_occupancy(n, m, h->fwd_smem, &h->fwd_ctas);
-  else bc_fwd_occupancy(S.dense, h->fwd_indirect, h->fwd_threads, h->fwd_smem, &h->fwd_ctas, 0);
+  else bc_fwd_occupancy(S.dense, h->fwd_indirect, h->fwd_threads, h->fwd_smem, &h->fwd_ctas, 0, fvg);
   if (h->fast_bwd) bc_bwdf_occupancy(n, h->bwd_threads, h->bwd_smem, &h->bwd_ctas);
-  else bc_bwd_occupancy(S.dense, h->bwd_threads, h->bwd_smem, &h->bwd_ctas, 0);
+  else bc_bwd_occupancy(S.dense, h->bwd_threads, h->bwd_smem, &h->bwd_ctas, 0, bvg);
   if (h->fwd_ctas < 1) h->fwd_ctas = 1;
   if (h->bwd_ctas < 1) h->bwd_ctas = 1;
-  if (h->fwd_small) { bc_fwd_occupancy(S.dense, 0, h->fwd_threads, h->fwd_smem, &h->fwd_ctas_small, 1); if (h->fwd_ctas_small <= h->fwd_ctas) h->fwd_small = 0; }
-  if (h->bwd_small) { bc_bwd_occupancy(S.dense, h->bwd_threads, h->bwd_smem, &h->bwd_ctas_small, 1); if (h->bwd_ctas_small <= h->bwd_ctas) h->bwd_small = 0; }
-  if (h->fwd_indirect || h->fwd_factor_global) h->fwd_ws_stride = bc_fwd_ws_doubles(n, m, h->fwd_factor_global);
+  if (h->fwd_small) { bc_fwd_occupancy(S.dense, 0, h->fwd_threads, h->fwd_smem, &h->fwd_ctas_small, 1, 0); if (h->fwd_ctas_small <= h->fwd_ctas) h->fwd_small = 0; }
+  if (h->bwd_small) { bc_bwd_occupancy(S.dense, h->bwd_threads, h->bwd_smem, &h->bwd_ctas_small, 1, 0); if (h->bwd_ctas_small <= h->bwd_ctas) h->bwd_small = 0; }
+  if (h->fwd_indirect || h->fwd_factor_global || fvg)
+    h->fwd_ws_stride = bc_fwd_ws_doubles(n, m, h->fwd_indirect || h->fwd_factor_global, h->fwd_factor_global, fvg ? d->nnzA : 0);
   if (h->bwd_vec_global && !h->fast_bwd) h->bwd_ws_stride = bc_bwd_ws_doubles(n, m, npoly);
   h->tma_ok = (d->nnzA > 0 && (d->nnzA % 2) == 0 && (size_t)d->nnzA * 8 < (1u << 20)) ? 1 : 0;
   // forward-mode derivative: the generic geometry (the backward's own when the backward is generic).  A structure without
   // one is still accepted; only bcone_jvp refuses it.
-  if (pick_generic(h->jvp_threads, h->jvp_smem, h->jvp_p_in_smem, h->jvp_vec_global) && bc_jvp_configure(S.dense, h->jvp_smem, 0) == cudaSuccess) {
+  if (pick_generic(h->jvp_threads, h->jvp_smem, h->jvp_p_in_smem, h->jvp_vec_global, h->jvp_vals_global) &&
+      bc_jvp_configure(S.dense, h->jvp_smem, 0, h->jvp_vals_global) == cudaSuccess) {
     h->jvp_ok = 1;
-    bc_jvp_occupancy(S.dense, h->jvp_threads, h->jvp_smem, &h->jvp_ctas, 0);
+    bc_jvp_occupancy(S.dense, h->jvp_threads, h->jvp_smem, &h->jvp_ctas, 0, h->jvp_vals_global);
     if (h->jvp_ctas < 1) h->jvp_ctas = 1;
-    h->jvp_small = h->small_mode != 0 && h->jvp_threads <= 256 && h->jvp_smem <= 56 * 1024 && bc_jvp_configure(S.dense, h->jvp_smem, 1) == cudaSuccess;
-    if (h->jvp_small) { bc_jvp_occupancy(S.dense, h->jvp_threads, h->jvp_smem, &h->jvp_ctas_small, 1); if (h->jvp_ctas_small <= h->jvp_ctas) h->jvp_small = 0; }
+    h->jvp_small = h->small_mode != 0 && !h->jvp_vals_global && h->jvp_threads <= 256 && h->jvp_smem <= 56 * 1024 && bc_jvp_configure(S.dense, h->jvp_smem, 1, 0) == cudaSuccess;
+    if (h->jvp_small) { bc_jvp_occupancy(S.dense, h->jvp_threads, h->jvp_smem, &h->jvp_ctas_small, 1, 0); if (h->jvp_ctas_small <= h->jvp_ctas) h->jvp_small = 0; }
     if (h->jvp_vec_global) h->jvp_ws_stride = bc_bwd_ws_doubles(n, m, npoly);
   }
   cudaGetLastError();   // (a refused configuration is not an error of this call)
@@ -593,8 +624,15 @@ extern "C" int bcone_solve_cached(void *handle, int32_t B, const double *A_vals,
   const size_t max_grid = (size_t)h->num_sms * std::max(h->fwd_ctas, h->fwd_ctas_small);
   Handle::StreamWs *sw = stream_ws(h, st);
   a.ws = nullptr; a.ws_stride = (long long)h->fwd_ws_stride; a.prof = h->prof;
-  if (h->fwd_indirect || h->fwd_factor_global) {
-    if (!ensure_slab(h, &sw->fwd, nullptr, h->fwd_ws_stride * max_grid)) return fail(h, BCONE_ENOMEM, "cudaMalloc forward workspace");
+  const int fvg = !h->fast_fwd && h->fwd_vals_global;
+  a.slab_vectors = h->fwd_indirect || h->fwd_factor_global;
+  if (h->fwd_indirect || h->fwd_factor_global || fvg) {
+    if (!ensure_slab(h, &sw->fwd, nullptr, h->fwd_ws_stride * max_grid)) {
+      char buf[160];
+      snprintf(buf, sizeof buf, "cudaMalloc forward workspace (%zu B: %zu B per CTA x %zu CTAs)", h->fwd_ws_stride * max_grid * sizeof(double),
+               h->fwd_ws_stride * sizeof(double), max_grid);
+      return fail(h, BCONE_ENOMEM, buf);
+    }
     a.ws = sw->fwd;
   }
   a.aa_ws = nullptr; a.aa_stride = 0;
@@ -611,7 +649,7 @@ extern "C" int bcone_solve_cached(void *handle, int32_t B, const double *A_vals,
   }
   CK(cudaMemsetAsync(ctr, 0, sizeof(int), st), "solve counter");
   if (h->fast_fwd) CK(bc_fwdf_launch(&a, grid, h->fwd_smem, st), "solve launch (fast)");
-  else CK(bc_fwd_launch(&a, h->fwd_indirect, grid, h->fwd_threads, h->fwd_smem, st, use_small), "solve launch");
+  else CK(bc_fwd_launch(&a, h->fwd_indirect, grid, h->fwd_threads, h->fwd_smem, st, use_small, fvg), "solve launch");
   h->launches++;
   return BCONE_OK;
 }
@@ -631,7 +669,8 @@ extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const do
   const int slot = h->slot++ % Handle::RING;
   int *ctr = h->counters + 4 * slot;
   a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
-  a.use_tma = h->tma_ok && (((uintptr_t)A_vals & 15) == 0); a.psd_total = h->psd_total; a.p_in_smem = h->p_in_smem;
+  // (values off chip: nothing of A is staged, use_tma only allows the bulk copy of P)
+  a.use_tma = h->bwd_vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = h->p_in_smem;
   CK(cudaSetDevice(h->device), "vjp set device");
   a.ws = nullptr; a.ws_stride = (long long)h->bwd_ws_stride;
   if (h->bwd_vec_global && !h->fast_bwd) {
@@ -663,7 +702,7 @@ extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const do
   const int use_small = h->bwd_small && (h->small_mode == 2 || B > h->num_sms * h->bwd_ctas);
   const int grid = std::min(B, h->num_sms * (use_small ? h->bwd_ctas_small : h->bwd_ctas));
   if (h->fast_bwd) CK(bc_bwdf_launch(&a, grid, h->bwd_threads, h->bwd_smem, st), "vjp launch (fast)");
-  else CK(bc_bwd_launch(&a, grid, h->bwd_threads, h->bwd_smem, st, use_small), "vjp launch");
+  else CK(bc_bwd_launch(&a, grid, h->bwd_threads, h->bwd_smem, st, use_small, h->bwd_vals_global), "vjp launch");
   h->launches++;
   return BCONE_OK;
 }
@@ -685,7 +724,7 @@ extern "C" int bcone_jvp(void *handle, int32_t B, const double *A_vals, const do
   int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
   a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
   if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // no block-preconditioned forward mode
-  a.use_tma = h->tma_ok && (((uintptr_t)A_vals & 15) == 0); a.psd_total = h->psd_total; a.p_in_smem = h->jvp_p_in_smem;
+  a.use_tma = h->jvp_vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = h->jvp_p_in_smem;
   CK(cudaSetDevice(h->device), "jvp set device");
   a.ws_stride = (long long)h->jvp_ws_stride;
   if (h->jvp_vec_global) {
@@ -697,7 +736,7 @@ extern "C" int bcone_jvp(void *handle, int32_t B, const double *A_vals, const do
   CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "jvp counter");
   const int use_small = h->jvp_small && (h->small_mode == 2 || B > h->num_sms * h->jvp_ctas);
   const int grid = std::min(B, h->num_sms * (use_small ? h->jvp_ctas_small : h->jvp_ctas));
-  CK(bc_jvp_launch(&a, grid, h->jvp_threads, h->jvp_smem, st, use_small), "jvp launch");
+  CK(bc_jvp_launch(&a, grid, h->jvp_threads, h->jvp_smem, st, use_small, h->jvp_vals_global), "jvp launch");
   h->launches++;
   return BCONE_OK;
 }
@@ -745,8 +784,12 @@ extern "C" int64_t bcone_launch_count(void *handle) { return handle ? ((Handle *
 extern "C" int bcone_path_info(void *handle, int32_t *fwd_path, int32_t *bwd_path) {
   Handle *h = (Handle *)handle;
   if (!h) return BCONE_EINVAL;
-  if (fwd_path) *fwd_path = h->fast_fwd ? 2 : (h->fwd_indirect ? 1 : (h->fwd_factor_global ? 3 : 0));
-  if (bwd_path) *bwd_path = h->block_bwd ? 2 : (h->fast_bwd ? 1 : 0);
+  if (fwd_path) {
+    if (h->fast_fwd) *fwd_path = 2;
+    else if (h->fwd_vals_global) *fwd_path = h->fwd_indirect ? 6 : (h->fwd_factor_global ? 5 : 4);
+    else *fwd_path = h->fwd_indirect ? 1 : (h->fwd_factor_global ? 3 : 0);
+  }
+  if (bwd_path) *bwd_path = h->block_bwd ? 2 : (h->fast_bwd ? 1 : (h->bwd_vals_global ? 3 : 0));
   return BCONE_OK;
 }
 

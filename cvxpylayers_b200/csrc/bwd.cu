@@ -7,7 +7,8 @@
 //   dA_ij = x_j r_{n+i} - pi_y,i r_j  on EVERY structural entry;  db = pi_y r_tau - r_y;
 //   dc = x r_tau - r_x;  dP_ij = (r_tau x_i - r_x,i) x_j (+ transpose term off the diagonal)
 // The instance's CSR values are staged once by TMA and stay in shared memory for all LSQR
-// iterations (each applies A and A' twice); P values are read from L2.
+// iterations (each applies A and A' twice); P values are read from L2.  Values that do not fit on chip are read in place from
+// A_vals instead (bwd_kernel<.., VG = true>).
 // The same kernel with JVP = true is the forward-mode derivative (bcone_jvp), the transpose of the above.
 #include "common.cuh"
 
@@ -23,19 +24,24 @@ __host__ __device__ inline size_t bwd_vec_doubles(int n, int m, int npoly) {
   return 3 * (size_t)n + 2 * (size_t)m + (m - npoly) + 7 * N + 2 * (size_t)m;
 }
 // vec_global: large instances keep the LSQR vectors in a per-CTA slab of global memory.
-__host__ __device__ inline size_t bwd_smem_doubles(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global) {
-  size_t d = 4 + (((size_t)nnzA + 1) & ~(size_t)1) + (((size_t)nnzP_smem + 1) & ~(size_t)1) + threads + 2 * 32;
+// vals_global: the CSR values are read in place from the caller's A_vals (instances whose values do not fit on chip).
+__host__ __device__ inline size_t bwd_smem_doubles(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
+                                                   int vals_global) {
+  size_t d = 4 + (vals_global ? 0 : ((size_t)nnzA + 1) & ~(size_t)1) + (((size_t)nnzP_smem + 1) & ~(size_t)1) + threads + 2 * 32;
   if (!vec_global) d += bwd_vec_doubles(n, m, npoly);
   if (max_psd > 0) d += psd_total + (size_t)(threads / 32) * (3 * (size_t)max_psd * max_psd + max_psd);
   return d + 9 * (size_t)nexp;
 }
 
+// VG: no shared memory for the values (M.Av is set per instance)
+template <bool VG = false>
 __device__ __forceinline__ void carve_b(BwdSmem &M, double *base, double *gws, int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp) {
   const int N = n + m + 1;
   double *q = base;
   M.bar = (uint64_t *)q; q += 2;
   M.ibuf = (int *)q; q += 2;
-  M.Av = q; q += (nnzA + 1) & ~1;
+  if (VG) M.Av = nullptr;
+  else { M.Av = q; q += (nnzA + 1) & ~1; }
   M.Pv = q; q += (nnzP_smem + 1) & ~1;
   M.part = q; q += threads; M.red = q; q += 2 * 32;
   double *v = gws ? gws : q;
@@ -299,15 +305,17 @@ __device__ __noinline__ void jvp_inactive_rows(const BwdArgs &a, const BwdSmem &
 //   g  = [-dA' pi_y - dc - dP x ; dA x - db ; pi_y'db + x'dc + x'dP x]   (tangents dA, dP, db, dc read from global memory)
 //   z  = LSQR(M, g);  dx = z_x - x z_tau,  dy = D z_y - y z_tau,  ds = D z_y - z_y - s z_tau
 // The adjoint's gradient assembly is G' and its dz is E'w, so it computes G' M^-T E'w; this computes E M^-1 G.
-template <bool DENSE, bool SMALL = false, bool JVP = false>   // SMALL: <= 256 threads, four resident CTAs per SM (see fwd.cu)
+// VG (values off chip): the instance's values are read in place from A_vals -- this kernel never writes them -- so nothing is
+// staged and shared memory holds only the vectors (when they fit) and the cone scratch.
+template <bool DENSE, bool SMALL = false, bool JVP = false, bool VG = false>   // SMALL: <= 256 threads, four resident CTAs per SM (see fwd.cu)
 __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(const __grid_constant__ BwdArgs a) {
   extern __shared__ __align__(16) double smem[];
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, N = n + m + 1, T = blockDim.x, t = threadIdx.x;
   const bcone_settings &st = a.st;
   BwdSmem M;
-  carve_b(M, smem, a.ws ? a.ws + (size_t)blockIdx.x * a.ws_stride : nullptr, n, m, S.z + S.l, S.nnzA, a.p_in_smem ? S.nnzP : 0, T, S.max_psd,
-          a.psd_total, S.ep + S.ed);
+  carve_b<VG>(M, smem, a.ws ? a.ws + (size_t)blockIdx.x * a.ws_stride : nullptr, n, m, S.z + S.l, S.nnzA, a.p_in_smem ? S.nnzP : 0, T, S.max_psd,
+              a.psd_total, S.ep + S.ed);
   if (t == 0) { mbar_init(M.bar, 1); fence_mbar_init(); }
   __syncthreads();
   uint32_t tma_phase = 0;
@@ -322,7 +330,14 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
     const double *Pglob = (a.P_vals && S.nnzP > 0) ? a.P_vals + (size_t)inst * S.nnzP : nullptr;
     const double *Pg = (Pglob && a.p_in_smem) ? M.Pv : Pglob;
     const bool tmaP = a.use_tma && Pglob && a.p_in_smem && (S.nnzP % 2 == 0) && (((uintptr_t)Pglob & 15) == 0);
-    if (a.use_tma) {
+    if constexpr (VG) {
+      M.Av = const_cast<double *>(Ag);   // (read only: the one store to M.Av is the staging below)
+      if (tmaP && t == 0) {
+        fence_proxy_async();
+        mbar_expect_tx(M.bar, (uint32_t)(S.nnzP * sizeof(double)));
+        tma_bulk_g2s(M.Pv, Pglob, (uint32_t)(S.nnzP * sizeof(double)), M.bar);
+      }
+    } else if (a.use_tma) {
       if (t == 0) {
         fence_proxy_async();
         mbar_expect_tx(M.bar, (uint32_t)((S.nnzA + (tmaP ? S.nnzP : 0)) * sizeof(double)));
@@ -345,7 +360,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
       M.piy[i] = (i >= S.z && i < S.z + S.l) ? fmax(vi, 0.0) : vi;
       if constexpr (!JVP) M.t1[i] = dyg[i];
     }
-    if (a.use_tma) { mbar_wait(M.bar, tma_phase); tma_phase ^= 1; }
+    if (VG ? tmaP : (bool)a.use_tma) { mbar_wait(M.bar, tma_phase); tma_phase ^= 1; }
     __syncthreads();
     // ---- cone Jacobian set-up: pi_y on SOC/PSD blocks, eigen-decompositions for PSD blocks ----
     if (S.ncones > 0) {
@@ -561,26 +576,29 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
   }
 }
 
-extern "C" size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global) {
-  return bwd_smem_doubles(n, m, npoly, nnzA, nnzP_smem, threads, max_psd, psd_total, nexp, vec_global) * sizeof(double);
+extern "C" size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
+                                    int vals_global) {
+  return bwd_smem_doubles(n, m, npoly, nnzA, nnzP_smem, threads, max_psd, psd_total, nexp, vec_global, vals_global) * sizeof(double);
 }
 extern "C" size_t bc_bwd_ws_doubles(int n, int m, int npoly) { return (bwd_vec_doubles(n, m, npoly) + 1) & ~(size_t)1; }
+// vg: the values-off-chip builds (512-thread only)
 #define BWD_DISPATCH(EXPR)                                                     \
   do {                                                                         \
-    if (small_cta) { if (dense) { auto k = bwd_kernel<true, true>; EXPR; } else { auto k = bwd_kernel<false, true>; EXPR; } } \
+    if (vg) { if (dense) { auto k = bwd_kernel<true, false, false, true>; EXPR; } else { auto k = bwd_kernel<false, false, false, true>; EXPR; } } \
+    else if (small_cta) { if (dense) { auto k = bwd_kernel<true, true>; EXPR; } else { auto k = bwd_kernel<false, true>; EXPR; } } \
     else { if (dense) { auto k = bwd_kernel<true, false>; EXPR; } else { auto k = bwd_kernel<false, false>; EXPR; } }         \
   } while (0)
-extern "C" cudaError_t bc_bwd_configure(int dense, size_t smem, int small_cta) {
+extern "C" cudaError_t bc_bwd_configure(int dense, size_t smem, int small_cta, int vg) {
   cudaError_t e = cudaSuccess;
   BWD_DISPATCH(e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   return e;
 }
-extern "C" cudaError_t bc_bwd_occupancy(int dense, int threads, size_t smem, int *ctas_per_sm, int small_cta) {
+extern "C" cudaError_t bc_bwd_occupancy(int dense, int threads, size_t smem, int *ctas_per_sm, int small_cta, int vg) {
   cudaError_t e = cudaSuccess;
   BWD_DISPATCH(e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, threads, smem));
   return e;
 }
-extern "C" cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta) {
+extern "C" cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta, int vg) {
   const int dense = a->S.dense;
   BWD_DISPATCH((k<<<grid, threads, smem, stream>>>(*a)));
   return cudaGetLastError();
@@ -588,20 +606,21 @@ extern "C" cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, si
 // forward-mode derivative: same kernel, same shared-memory layout, JVP = true
 #define JVP_DISPATCH(EXPR)                                                     \
   do {                                                                         \
-    if (small_cta) { if (dense) { auto k = bwd_kernel<true, true, true>; EXPR; } else { auto k = bwd_kernel<false, true, true>; EXPR; } } \
+    if (vg) { if (dense) { auto k = bwd_kernel<true, false, true, true>; EXPR; } else { auto k = bwd_kernel<false, false, true, true>; EXPR; } } \
+    else if (small_cta) { if (dense) { auto k = bwd_kernel<true, true, true>; EXPR; } else { auto k = bwd_kernel<false, true, true>; EXPR; } } \
     else { if (dense) { auto k = bwd_kernel<true, false, true>; EXPR; } else { auto k = bwd_kernel<false, false, true>; EXPR; } }         \
   } while (0)
-extern "C" cudaError_t bc_jvp_configure(int dense, size_t smem, int small_cta) {
+extern "C" cudaError_t bc_jvp_configure(int dense, size_t smem, int small_cta, int vg) {
   cudaError_t e = cudaSuccess;
   JVP_DISPATCH(e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   return e;
 }
-extern "C" cudaError_t bc_jvp_occupancy(int dense, int threads, size_t smem, int *ctas_per_sm, int small_cta) {
+extern "C" cudaError_t bc_jvp_occupancy(int dense, int threads, size_t smem, int *ctas_per_sm, int small_cta, int vg) {
   cudaError_t e = cudaSuccess;
   JVP_DISPATCH(e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, threads, smem));
   return e;
 }
-extern "C" cudaError_t bc_jvp_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta) {
+extern "C" cudaError_t bc_jvp_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta, int vg) {
   const int dense = a->S.dense;
   JVP_DISPATCH((k<<<grid, threads, smem, stream>>>(*a)));
   return cudaGetLastError();

@@ -60,6 +60,8 @@ struct FwdArgs {
   long long cache_stride;  // doubles per instance
   double *park;          // register-tiled kernel: per-CTA slab (4 x 8 x 512 doubles, L2) where the A tile waits out heavy cold calls
   int cache_reuse;       // 0: write the set-up of this solve; 1: A and P are unchanged since the solve that wrote it -> skip it
+  int slab_vectors;      // values-off-chip build (fwd_kernel<.., VG = true>): the vectors (and a direct solve's factor) follow the
+                         // values in the slab; 0 = they stay in shared memory
 };
 
 struct BwdArgs {

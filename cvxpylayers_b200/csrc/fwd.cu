@@ -2,7 +2,8 @@
 // (the work diffcp/SCS do for the reference at src/cvxpylayers/interfaces/diffcp_if.py:365,369;
 // rows F3-F6 of SURVEY.md section 8a).  One persistent CTA per instance; the instance's CSR
 // values (TMA bulk copy), the packed inverse Cholesky factor of the reduced normalised KKT
-// matrix and every iterate vector stay in shared memory for the whole solve.
+// matrix and every iterate vector stay in shared memory for the whole solve (larger instances: see the modes below and the
+// values-off-chip build, fwd_kernel<.., VG = true>).
 //
 // Per iteration (all on-chip):
 //   t_n  = rho_x w_x - A' w_y                         (transposed product, lanes across columns)
@@ -43,8 +44,9 @@ __host__ __device__ inline size_t fwd_part_doubles(int n, int threads) {   // (a
   const size_t d = (size_t)(8 * n > threads ? 8 * n : threads);
   return d > 272 ? d : 272;
 }
-__host__ __device__ inline size_t fwd_smem_doubles(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp) {
-  size_t nA = ((size_t)nnzA + 1) & ~(size_t)1;
+// vals_global: the CSR values live in the per-CTA slab instead (instances whose values do not fit next to the rest).
+__host__ __device__ inline size_t fwd_smem_doubles(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp, int vals_global) {
+  size_t nA = vals_global ? 0 : ((size_t)nnzA + 1) & ~(size_t)1;
   size_t d = 4 + nA + fwd_part_doubles(n, threads) + 8 * 32;
   if (!indirect) d += (size_t)n * (n + 1) / 2 + fwd_vec_doubles(n, m, 0);
   return d + cone_scratch_doubles(threads, max_psd, ns, nexp);
@@ -53,12 +55,16 @@ __host__ __device__ inline size_t fwd_smem_doubles(int n, int m, int nnzA, int t
 // gws != nullptr: the vectors live in the per-CTA global slab; li_global: the packed Cholesky factor follows them there
 // (mode 2: instances whose values fit on chip but whose factor does not -- the factor is then read from L2 / HBM twice per
 // iteration, which is still far cheaper than the conjugate-gradient solve of the indirect mode).
-__device__ __forceinline__ void carve(FwdSmem &M, double *base, double *gws, int n, int m, int nnzA, int threads, int max_psd, bool li_global = false) {
+// VG: the values are at `vals` (the front of the slab) and take no shared memory.
+template <bool VG = false>
+__device__ __forceinline__ void carve(FwdSmem &M, double *base, double *gws, int n, int m, int nnzA, int threads, int max_psd, bool li_global = false,
+                                      double *vals = nullptr) {
   const int N = n + m + 1;
   double *q = base;
   M.bar = (uint64_t *)q; q += 2;
   M.ibuf = (int *)q; q += 2;
-  M.Av = q; q += (nnzA + 1) & ~1;
+  if (VG) M.Av = vals;
+  else { M.Av = q; q += (nnzA + 1) & ~1; }
   M.part = q; q += fwd_part_doubles(n, threads); M.red = q; q += 8 * 32;
   if (!gws) { M.Li = q; q += n * (n + 1) / 2; } else M.Li = nullptr;
   double *v = gws ? gws : q;
@@ -257,14 +263,23 @@ __device__ bool factor_and_g(const FwdArgs &a, FwdSmem &M, const double *Pv, dou
 // SMALL: instances that run with <= 256 threads per CTA and a few tens of KB of shared memory are bound by the latency of one
 // CTA's dependent chain (barriers, reductions, a single projecting warp); compiled for four resident CTAs per SM (64 registers)
 // they overlap each other's stalls.  The large variant keeps 128 registers and one CTA of up to 512 threads per SM.
-template <bool DENSE, bool INDIRECT, bool SMALL = false>
+// VG (values off chip): instances whose CSR values do not fit in shared memory.  Each CTA copies the instance's values to the
+// front of its slab (Ruiz rescales them in place, the caller's A_vals stay untouched) and every product reads them from L2 / HBM;
+// the vectors and the factor stay on chip when they fit (a.slab_vectors = 0), else they follow the values in the slab.
+template <bool DENSE, bool INDIRECT, bool SMALL = false, bool VG = false>
 __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) fwd_kernel(const __grid_constant__ FwdArgs a) {
   extern __shared__ __align__(16) double smem[];
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, N = n + m + 1, T = blockDim.x, t = threadIdx.x;
   const bcone_settings &st = a.st;
   FwdSmem M;
-  carve(M, smem, a.ws ? a.ws + (size_t)blockIdx.x * a.ws_stride : nullptr, n, m, S.nnzA, T, S.max_psd, !INDIRECT && a.ws != nullptr);
+  if constexpr (VG) {
+    double *const slab = a.ws + (size_t)blockIdx.x * a.ws_stride;   // [values (even count: 16-byte aligned) | vectors | factor]
+    const bool vecs = INDIRECT || a.slab_vectors;
+    carve<true>(M, smem, vecs ? slab + ((S.nnzA + 1) & ~1) : nullptr, n, m, S.nnzA, T, S.max_psd, !INDIRECT && vecs, slab);
+  } else {
+    carve(M, smem, a.ws ? a.ws + (size_t)blockIdx.x * a.ws_stride : nullptr, n, m, S.nnzA, T, S.max_psd, !INDIRECT && a.ws != nullptr);
+  }
   if (t == 0) { mbar_init(M.bar, 1); fence_mbar_init(); }
   __syncthreads();
   uint32_t tma_phase = 0;
@@ -284,7 +299,16 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) fwd_kernel(c
     SUB_DECL(pi);
 
     // ---- stage the instance: one TMA bulk copy for the CSR values, plain loads for b, c ----
-    if (a.use_tma) {
+    if constexpr (VG) {   // values into the slab: 128-bit copies when the instance's row is 16-byte aligned
+      if ((((uintptr_t)Ag) & 15) == 0) {
+        const double2 *src = reinterpret_cast<const double2 *>(Ag);
+        double2 *dst = reinterpret_cast<double2 *>(M.Av);
+        for (int k = t; k < (S.nnzA >> 1); k += T) dst[k] = __ldg(src + k);
+        if ((S.nnzA & 1) && t == 0) M.Av[S.nnzA - 1] = __ldg(Ag + S.nnzA - 1);
+      } else {
+        for (int k = t; k < S.nnzA; k += T) M.Av[k] = __ldg(Ag + k);
+      }
+    } else if (a.use_tma) {
       if (t == 0) {
         fence_proxy_async();
         mbar_expect_tx(M.bar, (uint32_t)(S.nnzA * sizeof(double)));
@@ -296,7 +320,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) fwd_kernel(c
     double nb0 = 0, nc0 = 0;
     for (int i = t; i < m; i += T) { const double v = bg[i]; M.bh[i] = v; M.Dm[i] = 1.0; nb0 = fmax(nb0, fabs(v)); }
     for (int j = t; j < n; j += T) { const double v = cg[j]; M.ch[j] = v; M.En[j] = 1.0; nc0 = fmax(nc0, fabs(v)); }
-    if (a.use_tma) { mbar_wait(M.bar, tma_phase); tma_phase ^= 1; }
+    if (!VG && a.use_tma) { mbar_wait(M.bar, tma_phase); tma_phase ^= 1; }
     __syncthreads();
 
     pt.stamp(0);   // load
@@ -643,17 +667,25 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) fwd_kernel(c
 }
 
 // ----------------------------------------------------------------------------- host launcher
-extern "C" size_t bc_fwd_smem_bytes(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp) {
-  return fwd_smem_doubles(n, m, nnzA, threads, max_psd, indirect, ns, nexp) * sizeof(double);
+extern "C" size_t bc_fwd_smem_bytes(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp, int vals_global) {
+  return fwd_smem_doubles(n, m, nnzA, threads, max_psd, indirect, ns, nexp, vals_global) * sizeof(double);
 }
-// per-CTA slab: the vectors (+ the packed factor in mode 2)
-extern "C" size_t bc_fwd_ws_doubles(int n, int m, int with_factor) {
-  return ((fwd_vec_doubles(n, m, 1) + 1) & ~(size_t)1) + (with_factor ? (((size_t)n * (n + 1) / 2 + 1) & ~(size_t)1) : 0);
+// per-CTA slab: the values when they are off chip (nnzA_global > 0), then the vectors, then the packed factor
+extern "C" size_t bc_fwd_ws_doubles(int n, int m, int vectors, int with_factor, int nnzA_global) {
+  return (((size_t)nnzA_global + 1) & ~(size_t)1) + (vectors ? ((fwd_vec_doubles(n, m, 1) + 1) & ~(size_t)1) : 0) +
+         (with_factor ? (((size_t)n * (n + 1) / 2 + 1) & ~(size_t)1) : 0);
 }
 
+// vg: the values-off-chip builds (512-thread only: the tier serves large instances)
 #define FWD_DISPATCH(EXPR)                                        \
   do {                                                            \
-    if (small_cta && !indirect) {                                 \
+    if (vg) {                                                     \
+      if (dense && indirect) { auto k = fwd_kernel<true, true, false, true>; EXPR; }    \
+      else if (dense) { auto k = fwd_kernel<true, false, false, true>; EXPR; }        \
+      else if (indirect) { auto k = fwd_kernel<false, true, false, true>; EXPR; }     \
+      else { auto k = fwd_kernel<false, false, false, true>; EXPR; }                  \
+    }                                                             \
+    else if (small_cta && !indirect) {                            \
       if (dense) { auto k = fwd_kernel<true, false, true>; EXPR; }             \
       else { auto k = fwd_kernel<false, false, true>; EXPR; }                  \
     }                                                             \
@@ -663,17 +695,17 @@ extern "C" size_t bc_fwd_ws_doubles(int n, int m, int with_factor) {
     else { auto k = fwd_kernel<false, false>; EXPR; }                        \
   } while (0)
 
-extern "C" cudaError_t bc_fwd_configure(int dense, int indirect, size_t smem, int small_cta) {
+extern "C" cudaError_t bc_fwd_configure(int dense, int indirect, size_t smem, int small_cta, int vg) {
   cudaError_t e = cudaSuccess;
   FWD_DISPATCH(e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   return e;
 }
-extern "C" cudaError_t bc_fwd_occupancy(int dense, int indirect, int threads, size_t smem, int *ctas_per_sm, int small_cta) {
+extern "C" cudaError_t bc_fwd_occupancy(int dense, int indirect, int threads, size_t smem, int *ctas_per_sm, int small_cta, int vg) {
   cudaError_t e = cudaSuccess;
   FWD_DISPATCH(e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, threads, smem));
   return e;
 }
-extern "C" cudaError_t bc_fwd_launch(const FwdArgs *a, int indirect, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta) {
+extern "C" cudaError_t bc_fwd_launch(const FwdArgs *a, int indirect, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta, int vg) {
   const int dense = a->S.dense;
   FWD_DISPATCH((k<<<grid, threads, smem, stream>>>(*a)));
   return cudaGetLastError();

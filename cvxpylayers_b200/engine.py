@@ -131,9 +131,14 @@ class Engine:
         k = ["fwd_threads", "fwd_smem", "fwd_ctas_per_sm", "bwd_threads", "bwd_smem", "bwd_ctas_per_sm"]
         return {a: int(b.value) for a, b in zip(k, v)}
 
+    # codes 4-6 / 3: the values-off-chip tier (instances whose CSR values do not fit in shared memory; include/bcone.h)
     FWD_PATHS = ("fwd_kernel (on-chip Cholesky)", "fwd_kernel (indirect, CG)", "fwd_fast_kernel (register-tiled)",
-                 "fwd_kernel (values on chip, Cholesky factor and vectors in a global slab)")
-    BWD_PATHS = ("bwd_kernel (generic LSQR)", "bwd_fast_kernel (fused single-pass LSQR)", "bwd_block_kernel (KKT-block preconditioned, bwd_fast_kernel fallback)")
+                 "fwd_kernel (values on chip, Cholesky factor and vectors in a global slab)",
+                 "fwd_kernel (values off chip: values in a global slab, Cholesky factor and vectors on chip)",
+                 "fwd_kernel (values off chip: values, Cholesky factor and vectors in a global slab)",
+                 "fwd_kernel (values off chip: values and vectors in a global slab, indirect, CG)")
+    BWD_PATHS = ("bwd_kernel (generic LSQR)", "bwd_fast_kernel (fused single-pass LSQR)", "bwd_block_kernel (KKT-block preconditioned, bwd_fast_kernel fallback)",
+                 "bwd_kernel (generic LSQR, values off chip: read in place from A_vals)")
 
     def path_info(self) -> dict:
         f, b = C.c_int32(), C.c_int32()

@@ -196,23 +196,35 @@ def dense_lp(B: int, n: int, m: int, seed: int = 0) -> Batch:
     return Batch(st, A, b, c, None, x, y, s, f"dense_lp_n{n}_m{m}")
 
 
-def qp_as_socp(bt: Batch) -> Batch:
+def qp_as_socp(bt: Batch, factor: str = "cholesky") -> Batch:
     """The same QPs in the form the reference's DIFFCP path hands over: DIFFCP cannot take a quadratic objective
     (``src/cvxpylayers/_quad_form_dpp.py:29-32``: "DIFFCP decomposes quad_form to SOC"), so cvxpy
     canonicalises ``1/2 x'Px`` with ``P = R'R`` through an epigraph variable and one second-order cone of size n + 2,
 
         min c'x + t   s.t.  (original rows),   (t + 1, t - 1, sqrt2 R x) in SOC     [<=> x'Px <= 2t],
 
-    variables (x, t).  ``R`` is the upper-triangular Cholesky factor here (cvxpy's ``decomp_quad`` returns a dense factor of
-    the same product; with a dense n x n block the instance's values, 30,002 doubles at n = 100 / m = 200, exceed the 227 KB
-    a CTA can hold, the triangular factor's 25,052 fit).  Planted optimum carried over: t* = 1/2 x*'Px*, cone dual from the
-    KKT conditions."""
+    variables (x, t).  ``factor``:
+
+    * ``"cholesky"`` (default): ``R`` is the upper-triangular Cholesky factor, n (n + 1) / 2 values (25,052 values per instance
+      at n = 100 / m = 200: they fit in a CTA's shared memory);
+    * ``"eigen"``: cvxpy's own factor, ``decomp_quad``'s eigendecomposition ``P = V diag(lam) V'``, ``R = diag(sqrt(lam)) V'`` --
+      a dense n x n block (30,002 values at n = 100 / m = 200, more than a CTA holds: the engine's values-off-chip tier).
+
+    Planted optimum carried over (both factors: the formulas only use R'R = P): t* = 1/2 x*'Px*, cone dual from the KKT
+    conditions."""
     st = bt.structure
     n, m, B = st.n, st.m, bt.B
     assert st.P_indptr is not None and not st.cones.q and not st.cones.s
     Pd = np.stack([bt.P_dense(i) for i in range(B)])
-    R = np.swapaxes(np.linalg.cholesky(Pd), 1, 2)            # upper triangular, P = R'R
-    iu = np.triu_indices(n)
+    if factor == "cholesky":
+        R = np.swapaxes(np.linalg.cholesky(Pd), 1, 2)            # upper triangular, P = R'R
+        iu = np.triu_indices(n)
+    elif factor == "eigen":
+        lam, V = np.linalg.eigh(Pd)
+        R = np.sqrt(np.maximum(lam, 0.0))[:, :, None] * np.swapaxes(V, 1, 2)   # dense, P = R'R
+        iu = tuple(np.indices((n, n)).reshape(2, -1))
+    else:
+        raise ValueError(f"factor must be 'cholesky' or 'eigen', got {factor!r}")
     # rows: original m rows (columns 0..n-1), then SOC rows: [t+1], [t-1], sqrt2 R x
     rows, cols = [], []
     for i in range(m):
@@ -232,7 +244,7 @@ def qp_as_socp(bt: Batch) -> Batch:
     A_vals = np.ascontiguousarray(vals[:, order])
     b = np.concatenate([bt.b, np.ones((B, 1)), -np.ones((B, 1)), np.zeros((B, n))], axis=1)
     c = np.concatenate([bt.c, np.ones((B, 1))], axis=1)
-    out = Batch(st2, A_vals, b, c, None, name=bt.name + "_as_socp")
+    out = Batch(st2, A_vals, b, c, None, name=bt.name + ("_as_socp" if factor == "cholesky" else "_as_socp_eigen"))
     if bt.x_star is not None:
         x = bt.x_star
         Rx = np.einsum("bij,bj->bi", R, x)

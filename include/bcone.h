@@ -61,6 +61,13 @@ enum { BCONE_OK = 0, BCONE_EINVAL = -1, BCONE_ECUDA = -2, BCONE_ENOMEM = -3, BCO
 
 void bcone_default_settings(bcone_settings *st);
 
+/* Uploads the structure and picks the kernels (bcone_path_info).  The generic kernels keep an instance's CSR values in shared
+ * memory; when they do not fit next to the rest of a CTA's working set, the values stay in global memory (L2 when the grid's
+ * working set fits, HBM otherwise): the forward copies each instance's values into a per-CTA slab, the adjoint and the forward
+ * mode read them in place from A_vals.  That tier is tried only after every on-chip option has failed;
+ * BCONE_VALUES_GLOBAL=1 in the environment selects it for every generic kernel of a structure that would fit on chip (a test
+ * hook).  BCONE_EUNSUPPORTED: even then the on-chip scratch (per-warp PSD scratch and persistent eigenvectors, exp-cone slots,
+ * 8 n column partials) does not fit; the message names the largest PSD order that would have fit. */
 int bcone_create(const bcone_desc *desc, void **handle);
 void bcone_destroy(void *handle);
 const char *bcone_last_error(void *handle); /* handle may be NULL: last create() error */
@@ -203,8 +210,11 @@ int bcone_kernel_info(void *handle, int32_t *fwd_threads, int32_t *fwd_smem, int
                       int32_t *bwd_threads, int32_t *bwd_smem, int32_t *bwd_ctas_per_sm);
 /* Which kernels the structure selected.  fwd_path: 0 generic on-chip Cholesky (fwd.cu), 1 generic indirect (CG),
  * 2 register-tiled dense/polyhedral (fwd_fast.cu), 3 generic with the values on chip and the Cholesky factor + vectors in a
- * per-CTA slab of global memory (instances between the two; BCONE_FWD_MODE=indirect in the environment forces 1 instead).  bwd_path: 0 generic LSQR (bwd.cu), 1 fused single-pass LSQR
- * (bwd_fast.cu), 2 KKT-block preconditioned (bwd_block.cu, used when lsqr_precond = 2; falls back to 1 per instance). */
+ * per-CTA slab of global memory (instances between the two; BCONE_FWD_MODE=indirect in the environment forces 1 instead).
+ * Values off chip (see bcone_create): 4 values in the slab, Cholesky factor + vectors on chip; 5 values, Cholesky factor and
+ * vectors in the slab (n <= 512); 6 values + vectors in the slab, indirect (CG).  bwd_path: 0 generic LSQR (bwd.cu), 1 fused
+ * single-pass LSQR (bwd_fast.cu), 2 KKT-block preconditioned (bwd_block.cu, used when lsqr_precond = 2; falls back to 1 per
+ * instance), 3 generic LSQR with the values read in place from A_vals (values off chip; bcone_jvp then runs the same way). */
 int bcone_path_info(void *handle, int32_t *fwd_path, int32_t *bwd_path);
 
 #ifdef __cplusplus
