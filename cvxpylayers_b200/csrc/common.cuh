@@ -707,21 +707,29 @@ __device__ __forceinline__ void P_mul(const DevStruct &S, const double *Pv, cons
 // ----------------------------------------------------------------------------- packed Cholesky + inverse
 // In-place Cholesky K = L L' of a packed-lower SPD matrix (row i at i(i+1)/2) and in-place inverse X = L^{-1}:
 // the factor is applied afterwards as triangular / dense products, which keeps every solve free of sequential
-// substitution.  Everything advances FOUR columns / rows per step and is instruction-issue / latency bound with
-// 16 warps (tools/microbench.cu), so the design minimises warp-instructions and overlaps the serial chain:
+// substitution.  Everything advances EIGHT columns / rows per step and is latency / barrier bound with 16 warps
+// (tools/microbench.cu), so the design minimises steps and warp-instructions and overlaps the serial chain:
 //   * ONE sweep does both jobs.  Block row s of L is final (left of its diagonal) once panel s-1 is done, so its
 //     inverse step X_s = -M_s L_s X_{<s} runs inside factor step s: two barriers per step for both.
+//   * The diagonal block s is overwritten by M_s = L_ss^{-1} as soon as it is factored (nothing reads L_ss itself).
 //   * Phase A (thread-parallel): store X_{s-1} from the staging rows | panel s (one row per thread) |
 //     Z_s = -M_s L_s in place (one column per thread).
 //   * Phase B (warp-parallel, tensor cores): warp 0 updates the trailing tile that holds the next diagonal block
-//     and factors + inverts that 4 x 4 block right away (4 dependent rsqrt: the serial chain of the algorithm, one
-//     step ahead of everybody else); the other warps share the rank-4 trailing update (one DMMA per 8 x 8 tile,
-//     k = 4 is exactly the block width) and the inverse step (Z_s X_{<s}, one warp per 8 output columns, results to
-//     the staging rows).  The trailing work shrinks with s while the inverse work grows.
-// tmp: scratch of chol_scratch_doubles(n) doubles.  Block-uniform result (false: not positive definite).
-__host__ __device__ __forceinline__ int chol_scratch_doubles(int n) { return 26 * ((n + 3) >> 2) + 2; }
+//     and factors + inverts that 8 x 8 block right away (two 4 x 4 blocks with a 4 x 4 update between them: 8 dependent
+//     rsqrt, the serial chain of the algorithm, one step ahead of everybody else); the other warps share the rank-8
+//     trailing update (two DMMA k-steps on one accumulator per 8 x 8 tile) and the inverse step (Z_s X_{<s}: one 8 x 8
+//     output tile per warp).  The trailing work shrinks with s while the inverse work grows.
+//   * X_s cannot overwrite Z_s while other warps still read it, so its tiles wait for the next phase A: the first tile of
+//     each warp in that warp's registers, the rest (n > 8 x the phase-B warps) in staging rows.
+// tmp: scratch of chol_scratch_doubles(n, blockDim.x) doubles (staging rows + the pd flag).  Block-uniform result (false:
+// not positive definite).
+__host__ __device__ __forceinline__ int chol_held_cols(int threads) { return 8 * (threads > 32 ? (threads >> 5) - 1 : 1); }
+__host__ __device__ __forceinline__ int chol_scratch_doubles(int n, int threads) {
+  const int ld = 8 * ((n + 7) >> 3) - chol_held_cols(threads);
+  return 8 * (ld > 0 ? ld : 0) + 2;
+}
 // 1 / sqrt(x) for the Cholesky pivots: hardware approximation (2^-23) + two Newton steps (full double precision up to
-// a couple of ulp); roughly half the dependent latency of the library rsqrt, and four of them are chained per block.
+// a couple of ulp); roughly half the dependent latency of the library rsqrt, and eight of them are chained per block.
 __device__ __forceinline__ double rsqrt_nr(double x) {
   double y;
   asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
@@ -757,101 +765,141 @@ __device__ __forceinline__ Tri4 tri4_block(const double *K, int r0, int jb) {
   q.m31 = -fma(q.l32, q.m21, q.l31 * q.m11) * r3_; q.m32 = -q.l32 * q.m22 * r3_;
   return q;
 }
-#ifdef BC_CHOLPROF   // sub-phase cycle counters for tools/microbench.cu (thread 0, slots 16..24 of prof)
+#ifdef BC_CHOLPROF   // sub-phase cycle counters for tools/microbench.cu (thread 0, slots 17..20 of prof)
 #define CP_STAMP(k) if (prof && t == 0) { const long long now_ = clock64(); atomicAdd(prof + (k), (unsigned long long)(now_ - tt)); tt = now_; }
 #else
 #define CP_STAMP(k)
 #endif
-__device__ inline bool chol_inv_packed(double *K, int n, double *tmp, unsigned long long *prof = nullptr) {
+static __device__ __noinline__ bool chol_inv_packed(double *K, int n, double *tmp, unsigned long long *prof = nullptr) {
   const int T = blockDim.x, t = threadIdx.x, lane = t & 31, warp = t >> 5, nw = T >> 5;
-  const int nblk = (n + 3) >> 2, ld = 4 * nblk;
-  // scratch: 1 / L_kk | off-diagonal entries of the 4 x 4 inverses | staging rows of the inverse step | pd flag
-  double *isd = tmp, *moff = tmp + 4 * nblk, *Tst = tmp + 10 * nblk, *flag = tmp + 26 * nblk;
+  // inverse-step output columns [0, held) stay in registers (h0, h1: tile w0 of the warp, row fr, columns 8 w0 + 2 fc, + 1),
+  // the others wait in the staging rows
+  const int W = nw > 1 ? nw - 1 : 1, w0 = nw > 1 ? warp - 1 : 0, held = chol_held_cols(T);
+  const int lds = max(0, 8 * ((n + 7) >> 3) - held);
+  // scratch: staging rows of the inverse step | pd flag
+  double *Tst = tmp, *flag = tmp + 8 * lds;
+  double h0 = 0.0, h1 = 0.0;
   long long t0 = 0;
   if (prof && t == 0) t0 = clock64();
 #ifdef BC_CHOLPROF
   long long tt = t0;
 #endif
   const int fr = lane >> 2, fc = lane & 3;
-  // Diagonal block at J0 (warp 0, every lane computes, lane 0 publishes): L_D in place, its inverse in tmp.
+  auto rowp = [&](int i) { return K + ((i * (i + 1)) >> 1); };
+  // M (lane 0) over the jb x jb (jb <= 4) diagonal block at r0
+  auto put_m = [&](int r0, int jb, const Tri4 &q) {
+    double *D0 = rowp(r0) + r0;
+    D0[0] = q.m00;
+    if (jb > 1) { double *D1 = rowp(r0 + 1) + r0; D1[0] = q.m10; D1[1] = q.m11; }
+    if (jb > 2) { double *D2 = rowp(r0 + 2) + r0; D2[0] = q.m20; D2[1] = q.m21; D2[2] = q.m22; }
+    if (jb > 3) { double *D3 = rowp(r0 + 3) + r0; D3[0] = q.m30; D3[1] = q.m31; D3[2] = q.m32; D3[3] = q.m33; }
+  };
+  // Diagonal block at J0 (warp 0), replaced in place by its inverse M = L_D^{-1}:  L_D = [L11 0; L21 L22] with
+  // L11 L11' = D11, L21 = D21 M11', L22 L22' = D22 - L21 L21', and M21 = -M22 L21 M11.  The 4 x 4 blocks are factored by
+  // every lane (tri4_block); the 4 x 4 products take one entry (r, c) per lane of the first half-warp and meet in place.
   auto diag_block = [&](int J0) {
-    const int jb = min(4, n - J0);
-    const Tri4 q = tri4_block(K, J0, jb);
-    __syncwarp();   // every lane has read the block
-    if (lane == 0) {
-      double *D0 = K + ((J0 * (J0 + 1)) >> 1) + J0;
-      D0[0] = q.l00;
-      if (jb > 1) { double *D1 = K + (((J0 + 1) * (J0 + 2)) >> 1) + J0; D1[0] = q.l10; D1[1] = q.l11; }
-      if (jb > 2) { double *D2 = K + (((J0 + 2) * (J0 + 3)) >> 1) + J0; D2[0] = q.l20; D2[1] = q.l21; D2[2] = q.l22; }
-      if (jb > 3) { double *D3 = K + (((J0 + 3) * (J0 + 4)) >> 1) + J0; D3[0] = q.l30; D3[1] = q.l31; D3[2] = q.l32; D3[3] = q.l33; }
-      isd[J0] = q.m00; isd[J0 + 1] = q.m11; isd[J0 + 2] = q.m22; isd[J0 + 3] = q.m33;
-      double *mo = moff + 6 * (J0 >> 2);
-      mo[0] = q.m10; mo[1] = q.m20; mo[2] = q.m21; mo[3] = q.m30; mo[4] = q.m31; mo[5] = q.m32;
-      if (!q.pd) *flag = 0.0;
+    const int jb = min(8, n - J0), jb2 = jb - 4;
+    const Tri4 a = tri4_block(K, J0, min(4, jb));
+    bool pd = a.pd;
+    __syncwarp();   // every lane has read D11
+    if (lane == 0) put_m(J0, min(4, jb), a);
+    if (jb2 > 0) {
+      const int r = fr, c = fc;
+      const bool own = lane < 16 && r < jb2;
+      double *Rr = rowp(J0 + 4 + r) + J0;   // row 4 + r of the block
+      __syncwarp();   // M11 is in place
+      double v = 0.0;
+      if (own) {      // L21 = D21 M11'
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+          if (k <= c) v = fma(Rr[k], rowp(J0 + c)[J0 + k], v);
+      }
+      __syncwarp();   // every lane has read D21
+      if (own) Rr[c] = v;
+      __syncwarp();
+      if (own && c <= r) {   // D22 - L21 L21'
+        const double *Rc = rowp(J0 + 4 + c) + J0;
+        double g = Rr[4 + c];
+#pragma unroll
+        for (int k = 0; k < 4; k++) g = fma(-Rr[k], Rc[k], g);
+        Rr[4 + c] = g;
+      }
+      __syncwarp();
+      const Tri4 b = tri4_block(K, J0 + 4, jb2);
+      pd = pd && b.pd;
+      double u = 0.0;   // U = L21 M11
+      if (own) {
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+          if (k >= c) u = fma(Rr[k], rowp(J0 + k)[J0 + c], u);
+      }
+      __syncwarp();   // every lane has read D22 - L21 L21' and L21
+      if (lane == 0) put_m(J0 + 4, jb2, b);
+      __syncwarp();
+      double s = 0.0;   // M21 = -M22 U; U[k][c] is held by lane 4 k + c
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const double uk = __shfl_sync(0xffffffffu, u, 4 * k + c);
+        if (own && k <= r) s = fma(Rr[4 + k], uk, s);
+      }
+      if (own) Rr[c] = -s;
     }
+    if (lane == 0 && !pd) *flag = 0.0;
   };
   // One 8 x 8 tile (ta, tb), tb <= ta, of the trailing update K[i][j] -= sum_c L[i][J0+c] L[j][J0+c], i, j >= R0.
   auto trail_tile = [&](int ta, int tb, int J0, int jb, int R0) {
     const int ra = R0 + 8 * ta + fr, rb = R0 + 8 * tb + fr;
-    const double fa = (ra < n && fc < jb) ? -K[((ra * (ra + 1)) >> 1) + J0 + fc] : 0.0;
-    const double fb = (rb < n && fc < jb) ? K[((rb * (rb + 1)) >> 1) + J0 + fc] : 0.0;
+    const double *La = rowp(ra) + J0, *Lb = rowp(rb) + J0;
+    const double fa0 = (ra < n && fc < jb) ? -La[fc] : 0.0, fa1 = (ra < n && fc + 4 < jb) ? -La[fc + 4] : 0.0;
+    const double fb0 = (rb < n && fc < jb) ? Lb[fc] : 0.0, fb1 = (rb < n && fc + 4 < jb) ? Lb[fc + 4] : 0.0;
     const int cc = R0 + 8 * tb + 2 * fc;
-    double *pc = K + ((ra * (ra + 1)) >> 1) + cc;   // C entries (ra, cc), (ra, cc + 1)
+    double *pc = rowp(ra) + cc;   // C entries (ra, cc), (ra, cc + 1)
     const bool ok0 = ra < n && cc <= ra, ok1 = ra < n && cc + 1 <= ra;
     double c0 = ok0 ? pc[0] : 0.0, c1 = ok1 ? pc[1] : 0.0;
-    dmma884(c0, c1, fa, fb);
+    dmma884(c0, c1, fa0, fb0);
+    dmma884(c0, c1, fa1, fb1);
     if (ok0) pc[0] = c0;
     if (ok1) pc[1] = c1;
   };
-  // Inverse step of block row I0 (ib rows), output columns [8 jt, 8 jt + 8): (Z X_{<I0})[:, cols] into the staging rows.
+  // Inverse step of block row I0 (ib rows, I0 a multiple of 8), output columns [8 jt, 8 jt + 8): (Z X_{<I0})[:, cols]
+  // into registers (jt < W: the warp's first tile) or the staging rows.
   auto inv_tile = [&](int jt, int I0, int ib) {
     double c0 = 0.0, c1 = 0.0, d0 = 0.0, d1 = 0.0;
     const bool zr = fr < ib;
-    const double *zrow = K + (((I0 + (zr ? fr : 0)) * (I0 + (zr ? fr : 0) + 1)) >> 1);
+    const double *zrow = rowp(I0 + (zr ? fr : 0));
     const int jcol = 8 * jt + fr;
-    int k = 8 * jt;
-    // rows [8 jt, 8 jt + 8) of X meet the diagonal: triangular guard
-    for (int q = 0; q < 2 && k < I0; q++, k += 4) {
-      const int k0 = k + fc;
-      const double a0 = zr ? zrow[k0] : 0.0;
-      const double b0 = jcol <= k0 ? K[((k0 * (k0 + 1)) >> 1) + jcol] : 0.0;
-      if (q == 0) dmma884(c0, c1, a0, b0); else dmma884(d0, d1, a0, b0);
+    int k0 = 8 * jt + fc;
+    {  // rows [8 jt, 8 jt + 8) of X meet the diagonal: triangular guard
+      const double a0 = zr ? zrow[k0] : 0.0, a1 = zr ? zrow[k0 + 4] : 0.0;
+      const double b0 = jcol <= k0 ? rowp(k0)[jcol] : 0.0, b1 = jcol <= k0 + 4 ? rowp(k0 + 4)[jcol] : 0.0;
+      dmma884(c0, c1, a0, b0);
+      dmma884(d0, d1, a1, b1);
+      k0 += 8;
     }
     // full rows below: no guards, packed row offsets advanced incrementally, two accumulators in flight
-    int k0 = k + fc, o0 = ((k0 * (k0 + 1)) >> 1) + jcol;
-    for (; k + 8 <= I0; k += 8) {
+    int o0 = ((k0 * (k0 + 1)) >> 1) + jcol;
+    for (; k0 < I0; k0 += 8) {                         // (k0 - fc is a multiple of 8 and so is I0)
       const int o1 = o0 + 4 * k0 + 10;                 // row k0 + 4
       const double a0 = zr ? zrow[k0] : 0.0, a1 = zr ? zrow[k0 + 4] : 0.0;
       const double b0 = K[o0], b1 = K[o1];
       dmma884(c0, c1, a0, b0);
       dmma884(d0, d1, a1, b1);
-      o0 += 8 * k0 + 36; k0 += 8;                      // row k0 + 8
+      o0 += 8 * k0 + 36;                               // row k0 + 8
     }
-    if (k < I0) {                                      // one k-step left (I0 is a multiple of 4)
-      const double a0 = zr ? zrow[k0] : 0.0;
-      dmma884(c0, c1, a0, K[o0]);
-    }
-    if (fr < 4) {
-      const int col = 8 * jt + 2 * fc;
-      Tst[fr * ld + col] = c0 + d0; Tst[fr * ld + col + 1] = c1 + d1;   // col + 1 <= 8 jt + 7 < ld
+    if (jt < W) { h0 = c0 + d0; h1 = c1 + d1; }
+    else {
+      const int col = 8 * jt + 2 * fc - held;
+      Tst[fr * lds + col] = c0 + d0; Tst[fr * lds + col + 1] = c1 + d1;   // col + 1 <= 8 jt + 7 - held < lds
     }
   };
-  // X rows of block row I0 from the staging rows, and its diagonal block M
+  // X rows of block row I0 (left of the diagonal block, which already holds M) from the registers and the staging rows
   auto store_X = [&](int I0) {
-    const int ib = min(4, n - I0);
-    for (int j = (t + (T >> 1)) % T; j < I0; j += T) {   // (phase A runs three jobs: each starts on its own warps)
-      K[((I0 * (I0 + 1)) >> 1) + j] = Tst[j];
-      if (ib > 1) K[(((I0 + 1) * (I0 + 2)) >> 1) + j] = Tst[ld + j];
-      if (ib > 2) K[(((I0 + 2) * (I0 + 3)) >> 1) + j] = Tst[2 * ld + j];
-      if (ib > 3) K[(((I0 + 3) * (I0 + 4)) >> 1) + j] = Tst[3 * ld + j];
-    }
-    if (t == T - 1) {
-      const double *mo = moff + 6 * (I0 >> 2);
-      double *D0 = K + ((I0 * (I0 + 1)) >> 1) + I0;
-      D0[0] = isd[I0];
-      if (ib > 1) { double *D1 = K + (((I0 + 1) * (I0 + 2)) >> 1) + I0; D1[0] = mo[0]; D1[1] = isd[I0 + 1]; }
-      if (ib > 2) { double *D2 = K + (((I0 + 2) * (I0 + 3)) >> 1) + I0; D2[0] = mo[1]; D2[1] = mo[2]; D2[2] = isd[I0 + 2]; }
-      if (ib > 3) { double *D3 = K + (((I0 + 3) * (I0 + 4)) >> 1) + I0; D3[0] = mo[3]; D3[1] = mo[4]; D3[2] = mo[5]; D3[3] = isd[I0 + 3]; }
+    const int ib = min(8, n - I0);
+    if ((warp > 0 || nw == 1) && 8 * w0 < I0 && fr < ib) { double *p = rowp(I0 + fr) + 8 * w0 + 2 * fc; p[0] = h0; p[1] = h1; }
+    for (int j = held + (t + (T >> 1)) % T; j < I0; j += T) {   // (phase A runs three jobs: each starts on its own warps)
+#pragma unroll
+      for (int r = 0; r < 8; r++)
+        if (r < ib) rowp(I0 + r)[j] = Tst[r * lds + j - held];
     }
   };
   if (warp == 0) {
@@ -860,32 +908,44 @@ __device__ inline bool chol_inv_packed(double *K, int n, double *tmp, unsigned l
     diag_block(0);
   }
   __syncthreads();
-  for (int J0 = 0; J0 < n; J0 += 4) {
-    const int jb = min(4, n - J0), R0 = J0 + jb;
+  for (int J0 = 0; J0 < n; J0 += 8) {
+    const int jb = min(8, n - J0), R0 = J0 + jb;
     if (*flag == 0.0) return false;   // block-uniform: written before the last barrier
     // ---- phase A: X of the previous block row | panel | Z of this block row ----
-    if (J0 > 0) store_X(J0 - 4);
+    if (J0 > 0) store_X(J0 - 8);
     const int tz = (t + T - (T >> 2)) % T;   // Z starts at thread T / 4, the panel at thread 0, the X store at T / 2
     if (R0 + t < n || tz < J0) {
-      const double *mo = moff + 6 * (J0 >> 2);
-      const double m00 = isd[J0], m11 = isd[J0 + 1], m22 = isd[J0 + 2], m33 = isd[J0 + 3];
-      const double m10 = mo[0], m20 = mo[1], m21 = mo[2], m30 = mo[3], m31 = mo[4], m32 = mo[5];
+      const double *Md = rowp(J0) + J0;   // M = L_D^{-1}: entry (r, c) at Md[r (r + 1) / 2 + r J0 + c]
       for (int i = R0 + t; i < n; i += T) {   // panel: l_i = a_i L_D^{-T}
-        double *row = K + ((i * (i + 1)) >> 1) + J0;
-        const double a0 = row[0], a1 = jb > 1 ? row[1] : 0.0, a2 = jb > 2 ? row[2] : 0.0, a3 = jb > 3 ? row[3] : 0.0;
-        row[0] = a0 * m00;
-        if (jb > 1) row[1] = fma(a1, m11, a0 * m10);
-        if (jb > 2) row[2] = fma(a2, m22, fma(a1, m21, a0 * m20));
-        if (jb > 3) row[3] = fma(a3, m33, fma(a2, m32, fma(a1, m31, a0 * m30)));
+        double *row = rowp(i) + J0;
+        double a[8];
+#pragma unroll
+        for (int c = 0; c < 8; c++) a[c] = c < jb ? row[c] : 0.0;
+#pragma unroll
+        for (int c = 0; c < 8; c++) {
+          if (c < jb) {
+            const double *Mc = Md + ((c * (c + 1)) >> 1) + c * J0;
+            double s = 0.0;
+#pragma unroll
+            for (int k = 0; k <= c; k++) s = fma(a[k], Mc[k], s);
+            row[c] = s;
+          }
+        }
       }
-      double *L0 = K + ((J0 * (J0 + 1)) >> 1), *L1 = K + (((J0 + 1) * (J0 + 2)) >> 1), *L2 = K + (((J0 + 2) * (J0 + 3)) >> 1),
-             *L3 = K + (((J0 + 3) * (J0 + 4)) >> 1);
       for (int i = tz; i < J0; i += T) {      // Z = -M L on block row J0
-        const double a0 = L0[i], a1 = jb > 1 ? L1[i] : 0.0, a2 = jb > 2 ? L2[i] : 0.0, a3 = jb > 3 ? L3[i] : 0.0;
-        L0[i] = -(m00 * a0);
-        if (jb > 1) L1[i] = -fma(m11, a1, m10 * a0);
-        if (jb > 2) L2[i] = -fma(m22, a2, fma(m21, a1, m20 * a0));
-        if (jb > 3) L3[i] = -fma(m33, a3, fma(m32, a2, fma(m31, a1, m30 * a0)));
+        double a[8];
+#pragma unroll
+        for (int r = 0; r < 8; r++) a[r] = r < jb ? rowp(J0 + r)[i] : 0.0;
+#pragma unroll
+        for (int r = 0; r < 8; r++) {
+          if (r < jb) {
+            const double *Mr = Md + ((r * (r + 1)) >> 1) + r * J0;
+            double s = 0.0;
+#pragma unroll
+            for (int k = 0; k <= r; k++) s = fma(Mr[k], a[k], s);
+            rowp(J0 + r)[i] = -s;
+          }
+        }
       }
     }
     CP_STAMP(17);
@@ -894,14 +954,13 @@ __device__ inline bool chol_inv_packed(double *K, int n, double *tmp, unsigned l
     // ---- phase B: trailing update + next diagonal block | inverse step of this block row ----
     {
       const int ntl = R0 < n ? (n - R0 + 7) >> 3 : 0, ntile = (ntl * (ntl + 1)) >> 1;
-      const int ntj = (J0 + 7) >> 3;                   // inverse tiles (output columns < J0)
+      const int ntj = J0 >> 3;                         // inverse tiles (output columns < J0)
       if (warp == 0 && ntile > 0) {
         trail_tile(0, 0, J0, jb, R0);
         __syncwarp();
         diag_block(R0);
       }
       if (warp > 0 || nw == 1) {
-        const int W = nw > 1 ? nw - 1 : 1, w0 = nw > 1 ? warp - 1 : 0;
         const int nwork = ntj + (ntile > 0 ? ntile - 1 : 0);   // inverse tiles first (longest first), then trailing tiles 1..
         int ta = 0, tb = 0, e_cur = 0;
         for (int u = w0; u < nwork; u += W) {
@@ -920,7 +979,7 @@ __device__ inline bool chol_inv_packed(double *K, int n, double *tmp, unsigned l
     CP_STAMP(20);
   }
   if (*flag == 0.0) return false;
-  store_X(((n - 1) >> 2) << 2);
+  store_X(((n - 1) >> 3) << 3);
   __syncthreads();
   if (prof && t == 0) { const long long t1 = clock64(); atomicAdd(prof + 5, (unsigned long long)(t1 - t0)); }
   return true;

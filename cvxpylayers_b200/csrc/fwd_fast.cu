@@ -69,8 +69,11 @@ struct Geo {
   __host__ __device__ __forceinline__ int oVx() const { return oLi() + npk(); }
   __host__ __device__ __forceinline__ int oVy() const { return oVx() + 9 * npad(); }
   __host__ __device__ __forceinline__ int oRed() const { return oVy() + 7 * mpad(); }
-  __host__ __device__ __forceinline__ int oCh() const { return oRed() + 256 + 64; }   // Cholesky scratch (4 x 4 block inverses)
-  __host__ __device__ __forceinline__ int total() const { return oCh() + ((chol_scratch_doubles(npad()) + 1) & ~1); }
+  __host__ __device__ __forceinline__ int oCh() const { return oRed() + 256 + 64; }   // Cholesky scratch
+  // Its size, 26 ceil(npad / 4) + 2 doubles rounded up to even, is fixed so that the kernel's shared memory (and with it which
+  // shapes the kernel accepts) does not depend on the Cholesky routine; ok() checks that the routine's need at FT threads fits.
+  __host__ __device__ __forceinline__ int szCh() const { return (26 * ((npad() + 3) >> 2) + 3) & ~1; }
+  __host__ __device__ __forceinline__ int total() const { return oCh() + szCh(); }
   // cached set-up of one instance (global memory): [header 8 | E npad | D mpad | Kinv npad x kst]; header = {scale of the
   // stored Kinv, 1.0 once Kinv is stored, rho_x it was built with, ...}
   __host__ __device__ __forceinline__ int cE() const { return 8; }
@@ -78,7 +81,7 @@ struct Geo {
   __host__ __device__ __forceinline__ int cK() const { return cD() + mpad(); }
   __host__ __device__ __forceinline__ int cTotal() const { return (cK() + npad() * kst() + 1) & ~1; }
   __host__ __device__ __forceinline__ bool ok(int n, int m) const {
-    return n <= FT && m <= FT && CT() * RTu() <= FT && ((npad() + KR() - 1) / KR()) * CT() <= FT;
+    return n <= FT && m <= FT && CT() * RTu() <= FT && ((npad() + KR() - 1) / KR()) * CT() <= FT && chol_scratch_doubles(npad(), FT) <= szCh();
   }
 };
 
@@ -820,6 +823,9 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
         form_K(X, m, n, z, scale, st.rho_x, Li, Pg != nullptr, vx(VX_EN));
         SUB_STAMP(pf, 19);
         const bool okf = chol_cold(Li, n, sm + g.oCh());
+#ifdef BC_SUBPROF
+        if (a.prof && t == 0) atomicAdd(a.prof + 29, 1ull);   // factorisations (tools/phase_profile.py)
+#endif
         if (!okf) { if (t == 0) sc[SC_STATUS] = BCONE_FAILED; if (first) it = 0; break; }
         SUB_STAMP(pf, 21);
         // the tiles come back from the staged copy: nothing has to stay live across the factorisation

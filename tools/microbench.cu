@@ -307,7 +307,7 @@ __global__ void __launch_bounds__(512, 1) mb_kernel(Args a) {
     });
     if (c0 + c1 + f0 == 1.2345) a.out[t] = c0;
   }
-  // 15 (+ sub-phases 16..24): packed Cholesky + inverse of a 100 x 100 SPD matrix
+  // 15 (+ sub-phases 17..20): packed Cholesky + inverse of an n x n SPD matrix
   {
     for (int e = t; e < n * (n + 1) / 2; e += T) {
       int j = (int)((sqrtf(8.0f * e + 1.0f) - 1.0f) * 0.5f);
@@ -326,8 +326,9 @@ __global__ void __launch_bounds__(512, 1) mb_kernel(Args a) {
   if (t < m) a.out[1024 + t] = o1[t];
 }
 
-int main() {
-  const int m = 200, n = 100, reps = 200;
+int main(int argc, char **argv) {
+  const int m = 200, n = argc > 1 ? atoi(argv[1]) : 100, reps = 200;   // n: size of every product and of the Cholesky ledger
+  if (n < 2 || n > 128 || (n & 1)) { printf("n must be even, 2..128\n"); return 1; }
   std::vector<double> hA(m * n);
   for (int k = 0; k < m * n; k++) hA[k] = 0.001 * ((k * 7919) % 1000) - 0.5;
   Args a; a.m = m; a.n = n; a.reps = reps;
@@ -348,9 +349,11 @@ int main() {
                            "block_reduce<4>", "regtile rows", "regtile cols (100x50)", "regtile cols (quad)", "ruiz A sweep", "DMMA x128/thread", "K formation DMMA (x20)", "K formation 2x2 (x20)", ""};
   printf("smem %zu B\n", smem);
   for (int k = 0; k < 15; k++) printf("%-26s %10.1f cycles/call\n", names[k], (double)h[k] / grid / (k >= 13 ? 20 : reps));
-  const char *cn[10] = {"chol+inv total", "  F tri4 (factor)", "  F panel", "  F barrier 1", "  F trailing (DMMA)", "  F barrier 2", "  I tri4 (inverse)", "  I dot loop + shuffles",
-                        "  I barrier 1", "  I write + barrier 2"};
-  for (int k = 15; k < 25; k++) printf("%-26s %10.1f cycles/call\n", cn[k - 15], (double)h[k] / grid);
+  // slots 17..20 of chol_inv_packed, summed over its 8-column steps (thread 0's clock)
+  const char *cn[6] = {"chol+inv total", "", "  A: X store|panel|Z", "  barrier 1", "  B: trail+diag|inverse", "  barrier 2"};
+  printf("n = %d\n", n);
+  for (int k = 15; k < 21; k++)
+    if (k != 16) printf("%-26s %10.1f cycles/call\n", cn[k - 15], (double)h[k] / grid);
   printf("DMMA chain x64 (16 warps) %.1f, (1 warp) %.1f, DFMA chain x64 (1 warp) %.1f cycles/call\n", (double)h[25] / grid / reps, (double)h[26] / grid / reps, (double)h[27] / grid / reps);
   printf("chol check Linv[57][13]=%.12g  factor %.1f inverse %.1f\n", ho[2002], (double)h[5] / grid, (double)h[6] / grid);
   printf("check o2[3]=%g o1[5]=%g  K[57][13] dmma=%.12g 2x2=%.12g\n", ho[512 + 3], ho[1024 + 5], ho[2000], ho[2001]);

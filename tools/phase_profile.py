@@ -32,3 +32,5 @@ names = {5: "  [chol P] factor", 6: "  [chol P] inverse", 16: "  [eq] A sweep", 
 for k, nm in names.items():
     print(f"{nm:26s} {v[k]:10.0f} cycles/instance  {v[k] / MHZ:7.1f} us")
 print("fwd total us", v[:5].sum() / MHZ, "bwd total us", v[8:15].sum() / MHZ, "iters", sol.iters.float().mean().item())
+if v[29]:   # slot 29: a counter, not cycles (register-tiled forward only)
+    print("fwd factorisations per instance", v[29])
