@@ -46,9 +46,11 @@ cudaError_t bc_param_from_rows(const double *grows, const double *param, long lo
 cudaError_t bc_gather_cols(const double *in, long long ld, const int *map, const double *scale, int K, int B, int op, double *out, cudaStream_t st);
 cudaError_t bc_scatter_cols(const double *gout, const double *out, long long ld, const int *map, const double *scale, int K, int B, int op, double *gin, cudaStream_t st);
 cudaError_t bc_p2e(const double *p, const int *rptr, const int *cols, const double *vals, double *out, int K, int B, int ldo, int roff,
-                   const int *smap, const int *dmap, double sign, cudaStream_t st);
+                   const int *smap, const int *dmap, double sign, long long ldp, cudaStream_t st);
 cudaError_t bc_e2p(const double *in, const int *rptr, const int *cols, const double *vals, double *dp, int K, int B, int ldi, int roff,
-                   const int *smap, const int *dmap, double sign, int skip, cudaStream_t st);
+                   const int *smap, const int *dmap, double sign, int skip, long long ldp, cudaStream_t st);
+size_t bc_shared_part_doubles(const DevStruct *S, int B);
+cudaError_t bc_shared_grad(const DevStruct *S, const double *rec, const double *x, int B, double *dA, double *dP, double *part, cudaStream_t st);
 }
 
 namespace {
@@ -79,7 +81,10 @@ struct Handle {
   size_t fwd_ws_stride = 0, bwd_ws_stride = 0;
   // Per-stream scratch slabs (one per CTA of the grid): launches on different streams may overlap, launches on one
   // stream cannot, so the stream is the unit of ownership.  Allocated on first use.
-  struct StreamWs { cudaStream_t s; double *fwd = nullptr, *bwd = nullptr, *aa = nullptr, *park = nullptr, *jvp = nullptr; size_t aa_cap = 0; };
+  // shared matrices: setup = the batch's one set-up record of the register-tiled forward (+ the outputs of its set-up launch),
+  // srec / part = the adjoint's per-instance r, pi_y records and the reduction's partial sums (shared.cu)
+  struct StreamWs { cudaStream_t s; double *fwd = nullptr, *bwd = nullptr, *aa = nullptr, *park = nullptr, *jvp = nullptr; size_t aa_cap = 0;
+                    double *setup = nullptr, *srec = nullptr, *part = nullptr; size_t srec_cap = 0, part_cap = 0; };
   std::vector<StreamWs> sws;
   int block_bwd = 0, blk_threads = 0; size_t blk_smem = 0;   // KKT-block preconditioned backward (lsqr_precond = 2)
   int *fail_list[RING] = {nullptr}; int fail_cap[RING] = {0};
@@ -433,43 +438,60 @@ extern "C" int bcone_set_param_maps(void *handle, int32_t P1, const int32_t *A_p
   return BCONE_OK;
 }
 
-extern "C" int bcone_ingest_params(void *handle, int32_t B, const double *p_stack, double *A_vals, double *P_vals, double *b, double *c, void *stream) {
-  Handle *h = (Handle *)handle;
+// shared: A_vals / P_vals from column 0 of p_stack only (one copy for the batch), b and c from every column
+static int ingest_params(Handle *h, int32_t B, const double *p_stack, double *A_vals, double *P_vals, double *b, double *c, int shared, void *stream) {
   if (!h || B <= 0 || !p_stack || !A_vals || !b || !c) return fail(h, BCONE_EINVAL, "ingest_params: null argument");
   if (h->P1 <= 0) return fail(h, BCONE_EINVAL, "ingest_params: call bcone_set_param_maps first");
   cudaStream_t st = (cudaStream_t)stream;
   const DevStruct &S = h->S;
-  CK(bc_p2e(p_stack, h->pmA.ptr, h->pmA.col, h->pmA.val, A_vals, S.nnzA, B, S.nnzA, 0, h->d_gather, nullptr, -1.0, st), "ingest_params A");
+  const int BM = shared ? 1 : B;   // instances of the matrix values
+  CK(bc_p2e(p_stack, h->pmA.ptr, h->pmA.col, h->pmA.val, A_vals, S.nnzA, BM, S.nnzA, 0, h->d_gather, nullptr, -1.0, B, st), "ingest_params A");
   CK(cudaMemsetAsync(b, 0, (size_t)B * S.m * sizeof(double), st), "ingest_params b memset");
-  CK(bc_p2e(p_stack, h->pmA.ptr, h->pmA.col, h->pmA.val, b, h->nb, B, S.m, S.nnzA, nullptr, h->d_bidx, 1.0, st), "ingest_params b");
-  CK(bc_p2e(p_stack, h->pmq.ptr, h->pmq.col, h->pmq.val, c, S.n, B, S.n, 0, nullptr, nullptr, 1.0, st), "ingest_params c");
+  CK(bc_p2e(p_stack, h->pmA.ptr, h->pmA.col, h->pmA.val, b, h->nb, B, S.m, S.nnzA, nullptr, h->d_bidx, 1.0, B, st), "ingest_params b");
+  CK(bc_p2e(p_stack, h->pmq.ptr, h->pmq.col, h->pmq.val, c, S.n, B, S.n, 0, nullptr, nullptr, 1.0, B, st), "ingest_params c");
   h->launches += 3;
   if (P_vals && S.nnzP > 0) {
     if (!h->pmP.rows) return fail(h, BCONE_EINVAL, "ingest_params: structure has P but no parameter map for it");
-    CK(bc_p2e(p_stack, h->pmP.ptr, h->pmP.col, h->pmP.val, P_vals, S.nnzP, B, S.nnzP, 0, h->d_gatherP, nullptr, 1.0, st), "ingest_params P");
+    CK(bc_p2e(p_stack, h->pmP.ptr, h->pmP.col, h->pmP.val, P_vals, S.nnzP, BM, S.nnzP, 0, h->d_gatherP, nullptr, 1.0, B, st), "ingest_params P");
     h->launches++;
   }
   return BCONE_OK;
 }
+extern "C" int bcone_ingest_params(void *handle, int32_t B, const double *p_stack, double *A_vals, double *P_vals, double *b, double *c, void *stream) {
+  return ingest_params((Handle *)handle, B, p_stack, A_vals, P_vals, b, c, 0, stream);
+}
+extern "C" int bcone_ingest_params_shared(void *handle, int32_t B, const double *p_stack, double *A_vals, double *P_vals, double *b, double *c,
+                                          void *stream) {
+  return ingest_params((Handle *)handle, B, p_stack, A_vals, P_vals, b, c, 1, stream);
+}
 
-extern "C" int bcone_emit_params(void *handle, int32_t B, const double *dA_vals, const double *dP_vals, const double *db, const double *dc,
-                                 double *dp_stack, void *stream) {
-  Handle *h = (Handle *)handle;
+// shared: dA_vals / dP_vals are the batch sums [nnzA] / [nnzP], written into column 0 of dp_stack; db, dc into every column
+static int emit_params(Handle *h, int32_t B, const double *dA_vals, const double *dP_vals, const double *db, const double *dc, double *dp_stack,
+                       int shared, void *stream) {
   if (!h || B <= 0 || !dA_vals || !db || !dc || !dp_stack) return fail(h, BCONE_EINVAL, "emit_params: null argument");
   if (h->P1 <= 0) return fail(h, BCONE_EINVAL, "emit_params: call bcone_set_param_maps first");
   cudaStream_t st = (cudaStream_t)stream;
   const DevStruct &S = h->S;
   const int skip = h->P1 - 1;   // the constant-1 row of p_stack is not a parameter
   CK(cudaMemsetAsync(dp_stack, 0, (size_t)h->P1 * B * sizeof(double), st), "emit_params memset");
-  CK(bc_e2p(dA_vals, h->pmA.ptr, h->pmA.col, h->pmA.val, dp_stack, S.nnzA, B, S.nnzA, 0, nullptr, h->d_gather, -1.0, skip, st), "emit_params dA");
-  CK(bc_e2p(db, h->pmA.ptr, h->pmA.col, h->pmA.val, dp_stack, h->nb, B, S.m, S.nnzA, h->d_bidx, nullptr, 1.0, skip, st), "emit_params db");
-  CK(bc_e2p(dc, h->pmq.ptr, h->pmq.col, h->pmq.val, dp_stack, S.n, B, S.n, 0, nullptr, nullptr, 1.0, skip, st), "emit_params dc");
+  const int BM = shared ? 1 : B;
+  CK(bc_e2p(dA_vals, h->pmA.ptr, h->pmA.col, h->pmA.val, dp_stack, S.nnzA, BM, S.nnzA, 0, nullptr, h->d_gather, -1.0, skip, B, st), "emit_params dA");
+  CK(bc_e2p(db, h->pmA.ptr, h->pmA.col, h->pmA.val, dp_stack, h->nb, B, S.m, S.nnzA, h->d_bidx, nullptr, 1.0, skip, B, st), "emit_params db");
+  CK(bc_e2p(dc, h->pmq.ptr, h->pmq.col, h->pmq.val, dp_stack, S.n, B, S.n, 0, nullptr, nullptr, 1.0, skip, B, st), "emit_params dc");
   h->launches += 3;
   if (dP_vals && S.nnzP > 0 && h->pmP.rows) {
-    CK(bc_e2p(dP_vals, h->pmP.ptr, h->pmP.col, h->pmP.val, dp_stack, S.nnzP, B, S.nnzP, 0, nullptr, h->d_gatherP, 1.0, skip, st), "emit_params dP");
+    CK(bc_e2p(dP_vals, h->pmP.ptr, h->pmP.col, h->pmP.val, dp_stack, S.nnzP, BM, S.nnzP, 0, nullptr, h->d_gatherP, 1.0, skip, B, st), "emit_params dP");
     h->launches++;
   }
   return BCONE_OK;
+}
+extern "C" int bcone_emit_params(void *handle, int32_t B, const double *dA_vals, const double *dP_vals, const double *db, const double *dc,
+                                 double *dp_stack, void *stream) {
+  return emit_params((Handle *)handle, B, dA_vals, dP_vals, db, dc, dp_stack, 0, stream);
+}
+extern "C" int bcone_emit_params_shared(void *handle, int32_t B, const double *dA_sum, const double *dP_sum, const double *db, const double *dc,
+                                        double *dp_stack, void *stream) {
+  return emit_params((Handle *)handle, B, dA_sum, dP_sum, db, dc, dp_stack, 1, stream);
 }
 
 extern "C" int bcone_ingest_pitched(void *handle, int32_t B, int64_t ldb, const double *A_eval, const double *q_eval, const double *P_eval,
@@ -596,10 +618,11 @@ extern "C" int bcone_solve(void *handle, int32_t B, const double *A_vals, const 
                            double *resid, const bcone_settings *stg, void *stream) {
   return bcone_solve_warm(handle, B, A_vals, P_vals, b, c, nullptr, nullptr, nullptr, x, y, s, status, iters, resid, stg, stream);
 }
-extern "C" int bcone_solve_cached(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
-                                  const double *x0, const double *y0, const double *s0, double *x, double *y, double *s, int32_t *status,
-                                  int32_t *iters, double *resid, void *cache, int32_t reuse, const bcone_settings *stg, void *stream) {
-  Handle *h = (Handle *)handle;
+// shared: A_vals [nnzA] / P_vals [nnzP] are one copy for the whole batch (stride 0); with the register-tiled kernel the batch
+// then also shares one set-up (caller's cache must be NULL)
+static int solve_impl(Handle *h, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                      const double *x0, const double *y0, const double *s0, double *x, double *y, double *s, int32_t *status,
+                      int32_t *iters, double *resid, void *cache, int32_t reuse, int shared, const bcone_settings *stg, void *stream) {
   if (h && cache && !h->fast_fwd) return fail(h, BCONE_EINVAL, "solve: this structure has no cached set-up path (bcone_cache_bytes() is 0)");
   if (h && cache && ((uintptr_t)cache & 15)) return fail(h, BCONE_EINVAL, "solve: cache must be 16-byte aligned");
   if (h && ((x0 != nullptr) != (y0 != nullptr) || (x0 != nullptr) != (s0 != nullptr))) return fail(h, BCONE_EINVAL, "solve: warm start needs x0, y0 and s0 together");
@@ -615,6 +638,7 @@ extern "C" int bcone_solve_cached(void *handle, int32_t B, const double *A_vals,
   a.x = x; a.y = y; a.s = s; a.status = status; a.iters = iters; a.resid = resid; a.st = *stg;
   a.x0 = x0; a.y0 = y0; a.s0 = s0;
   a.cache = (double *)cache; a.cache_stride = h->fast_fwd ? (long long)bc_fwdf_cache_doubles(h->S.n, h->S.m) : 0; a.cache_reuse = cache && reuse;
+  a.sA = shared ? 0 : h->S.nnzA; a.sP = shared ? 0 : h->S.nnzP;
   int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
   a.counter = ctr; a.use_tma = h->tma_ok && (((uintptr_t)A_vals & 15) == 0);
   // the 4-CTA/SM build only when the batch does not fit the resident capacity of the 128-register build
@@ -647,18 +671,47 @@ extern "C" int bcone_solve_cached(void *handle, int32_t B, const double *A_vals,
     if (!ensure_slab(h, &sw->park, nullptr, (size_t)32 * 512 * max_grid)) return fail(h, BCONE_ENOMEM, "cudaMalloc tile parking slab");
     a.park = sw->park;
   }
+  if (shared && h->fast_fwd) {
+    // One set-up for the batch: a launch of one CTA builds the record (E, D, K^-1 at the initial scale) by the cached set-up's
+    // own code -- it stops after the first iteration, so the record is never refreshed at another scale -- and the batch
+    // reads it with record stride 0, as with reuse = 1.  Its solution of instance 0 goes to scratch behind the record.
+    const size_t rec = bc_fwdf_cache_doubles(h->S.n, h->S.m), extra = (size_t)h->S.n + 2 * (size_t)h->S.m + 4;
+    if (!ensure_slab(h, &sw->setup, nullptr, rec + extra)) return fail(h, BCONE_ENOMEM, "cudaMalloc shared set-up record");
+    FwdArgs u = a;
+    double *o = sw->setup + rec;
+    u.B = 1; u.x0 = u.y0 = u.s0 = nullptr; u.x = o; u.y = o + h->S.n; u.s = o + h->S.n + h->S.m; u.resid = nullptr;
+    u.status = (int *)(o + h->S.n + 2 * h->S.m); u.iters = u.status + 2;
+    u.st.max_iters = 1; u.st.acceleration_lookback = 0; u.aa_ws = nullptr; u.aa_stride = 0;
+    u.cache = sw->setup; u.cache_stride = (long long)rec; u.cache_reuse = 0;
+    int *uctr = h->counters + 4 * (h->slot++ % Handle::RING);
+    u.counter = uctr;
+    CK(cudaMemsetAsync(uctr, 0, sizeof(int), st), "solve counter (set-up)");
+    CK(bc_fwdf_launch(&u, 1, h->fwd_smem, st), "solve launch (shared set-up)");
+    h->launches++;
+    a.cache = sw->setup; a.cache_stride = 0; a.cache_reuse = 1;
+  }
   CK(cudaMemsetAsync(ctr, 0, sizeof(int), st), "solve counter");
   if (h->fast_fwd) CK(bc_fwdf_launch(&a, grid, h->fwd_smem, st), "solve launch (fast)");
   else CK(bc_fwd_launch(&a, h->fwd_indirect, grid, h->fwd_threads, h->fwd_smem, st, use_small, fvg), "solve launch");
   h->launches++;
   return BCONE_OK;
 }
+extern "C" int bcone_solve_cached(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                                  const double *x0, const double *y0, const double *s0, double *x, double *y, double *s, int32_t *status,
+                                  int32_t *iters, double *resid, void *cache, int32_t reuse, const bcone_settings *stg, void *stream) {
+  return solve_impl((Handle *)handle, B, A_vals, P_vals, b, c, x0, y0, s0, x, y, s, status, iters, resid, cache, reuse, 0, stg, stream);
+}
+extern "C" int bcone_solve_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                                  const double *x0, const double *y0, const double *s0, double *x, double *y, double *s, int32_t *status,
+                                  int32_t *iters, double *resid, const bcone_settings *stg, void *stream) {
+  return solve_impl((Handle *)handle, B, A_vals, P_vals, b, c, x0, y0, s0, x, y, s, status, iters, resid, nullptr, 0, 1, stg, stream);
+}
 
-extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b,
-                         const double *c, const double *x, const double *y, const double *s, const double *dx,
-                         const double *dy, double *dA_vals, double *dP_vals, double *db, double *dc,
-                         int32_t *lsqr_iters, const bcone_settings *stg, void *stream) {
-  Handle *h = (Handle *)handle;
+// shared: A_vals / P_vals one copy for the batch; dA_vals [nnzA] / dP_vals [nnzP] receive the batch sums
+static int vjp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_vals, const double *b,
+                    const double *c, const double *x, const double *y, const double *s, const double *dx,
+                    const double *dy, double *dA_vals, double *dP_vals, double *db, double *dc,
+                    int32_t *lsqr_iters, int shared, const bcone_settings *stg, void *stream) {
   if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !dx || !dy || !dA_vals || !db || !dc || !stg)
     return fail(h, BCONE_EINVAL, "vjp: null argument");
   if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "vjp: structure has P but P_vals is NULL");
@@ -666,6 +719,23 @@ extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const do
   BwdArgs a;
   a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
   a.x = x; a.y = y; a.s = s; a.dx = dx; a.dy = dy; a.dA = dA_vals; a.dP = dP_vals; a.db = db; a.dc = dc;
+  a.sA = shared ? 0 : h->S.nnzA; a.sP = shared ? 0 : h->S.nnzP; a.srec = nullptr;
+  a.tA = a.tP = a.tb = a.tc = nullptr; a.tx = a.ty = a.ts = nullptr;
+  Handle::StreamWs *sw = stream_ws(h, st);
+  if (shared) {
+    const size_t R = (size_t)bc_srec_doubles(h->S.n, h->S.m);
+    if (!ensure_slab(h, &sw->srec, &sw->srec_cap, R * B) || !ensure_slab(h, &sw->part, &sw->part_cap, bc_shared_part_doubles(&h->S, B)))
+      return fail(h, BCONE_ENOMEM, "cudaMalloc shared-matrix adjoint scratch");
+    a.srec = sw->srec; a.dA = nullptr; a.dP = nullptr;
+  }
+  // batch-summed dA / dP from the records (same stream: after the kernels that wrote them)
+  auto reduce = [&]() -> int {
+    if (shared) {
+      CK(bc_shared_grad(&h->S, sw->srec, x, B, dA_vals, h->S.nnzP > 0 ? dP_vals : nullptr, sw->part, st), "vjp shared reduction");
+      h->launches += (h->S.nnzA > 0 ? 2 : 0) + (h->S.nnzP > 0 && dP_vals ? 2 : 0);   // two stages per matrix
+    }
+    return BCONE_OK;
+  };
   const int slot = h->slot++ % Handle::RING;
   int *ctr = h->counters + 4 * slot;
   a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
@@ -674,7 +744,6 @@ extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const do
   CK(cudaSetDevice(h->device), "vjp set device");
   a.ws = nullptr; a.ws_stride = (long long)h->bwd_ws_stride;
   if (h->bwd_vec_global && !h->fast_bwd) {
-    Handle::StreamWs *sw = stream_ws(h, st);
     if (!ensure_slab(h, &sw->bwd, nullptr, h->bwd_ws_stride * (size_t)h->num_sms * std::max(h->bwd_ctas, h->bwd_ctas_small))) return fail(h, BCONE_ENOMEM, "cudaMalloc backward workspace");
     a.ws = sw->bwd;
   }
@@ -695,7 +764,7 @@ extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const do
     f.fail_list = nullptr; f.fail_count = nullptr;
     CK(bc_bwdf_launch(&f, std::min(B, h->num_sms * h->bwd_ctas), h->bwd_threads, h->bwd_smem, st), "vjp launch (fallback)");
     h->launches += 2;
-    return BCONE_OK;
+    return reduce();
   }
   if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // block factorisation not available for this structure
   CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "vjp counter");
@@ -704,14 +773,26 @@ extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const do
   if (h->fast_bwd) CK(bc_bwdf_launch(&a, grid, h->bwd_threads, h->bwd_smem, st), "vjp launch (fast)");
   else CK(bc_bwd_launch(&a, grid, h->bwd_threads, h->bwd_smem, st, use_small, h->bwd_vals_global), "vjp launch");
   h->launches++;
-  return BCONE_OK;
+  return reduce();
+}
+extern "C" int bcone_vjp(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b,
+                         const double *c, const double *x, const double *y, const double *s, const double *dx,
+                         const double *dy, double *dA_vals, double *dP_vals, double *db, double *dc,
+                         int32_t *lsqr_iters, const bcone_settings *stg, void *stream) {
+  return vjp_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, dx, dy, dA_vals, dP_vals, db, dc, lsqr_iters, 0, stg, stream);
+}
+extern "C" int bcone_vjp_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b,
+                                const double *c, const double *x, const double *y, const double *s, const double *dx,
+                                const double *dy, double *dA_sum, double *dP_sum, double *db, double *dc,
+                                int32_t *lsqr_iters, const bcone_settings *stg, void *stream) {
+  return vjp_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, dx, dy, dA_sum, dP_sum, db, dc, lsqr_iters, 1, stg, stream);
 }
 
-extern "C" int bcone_jvp(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
-                         const double *x, const double *y, const double *s, const double *dA_vals, const double *dP_vals,
-                         const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters,
-                         const bcone_settings *stg, void *stream) {
-  Handle *h = (Handle *)handle;
+// shared: A_vals / P_vals and the tangents dA_vals / dP_vals are one copy for the batch
+static int jvp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                    const double *x, const double *y, const double *s, const double *dA_vals, const double *dP_vals,
+                    const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters, int shared,
+                    const bcone_settings *stg, void *stream) {
   if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !dA_vals || !db || !dc || !dx || !dy || !stg)
     return fail(h, BCONE_EINVAL, "jvp: null argument");
   if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "jvp: structure has P but P_vals is NULL");
@@ -721,6 +802,7 @@ extern "C" int bcone_jvp(void *handle, int32_t B, const double *A_vals, const do
   a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
   a.x = x; a.y = y; a.s = s;
   a.tA = dA_vals; a.tP = h->S.nnzP > 0 ? dP_vals : nullptr; a.tb = db; a.tc = dc; a.tx = dx; a.ty = dy; a.ts = ds;
+  a.sA = shared ? 0 : h->S.nnzA; a.sP = shared ? 0 : h->S.nnzP;
   int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
   a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
   if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // no block-preconditioned forward mode
@@ -739,6 +821,18 @@ extern "C" int bcone_jvp(void *handle, int32_t B, const double *A_vals, const do
   CK(bc_jvp_launch(&a, grid, h->jvp_threads, h->jvp_smem, st, use_small, h->jvp_vals_global), "jvp launch");
   h->launches++;
   return BCONE_OK;
+}
+extern "C" int bcone_jvp(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                         const double *x, const double *y, const double *s, const double *dA_vals, const double *dP_vals,
+                         const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters,
+                         const bcone_settings *stg, void *stream) {
+  return jvp_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, dA_vals, dP_vals, db, dc, dx, dy, ds, lsqr_iters, 0, stg, stream);
+}
+extern "C" int bcone_jvp_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                                const double *x, const double *y, const double *s, const double *dA, const double *dP,
+                                const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters,
+                                const bcone_settings *stg, void *stream) {
+  return jvp_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, dA, dP, db, dc, dx, dy, ds, lsqr_iters, 1, stg, stream);
 }
 
 // Strided host<->device copy on the caller's stream (cudaMemcpy2DAsync): lets the reference-facing

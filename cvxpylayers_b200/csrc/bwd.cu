@@ -265,8 +265,8 @@ template <bool DENSE>
 __device__ __noinline__ double jvp_rhs(const BwdArgs &a, const BwdSmem &M, int inst, const ColPlan &plA, const ColPlan &plN) {
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, T = blockDim.x, t = threadIdx.x;
-  const double *tAg = a.tA + (size_t)inst * S.nnzA, *tbg = a.tb + (size_t)inst * m, *tcg = a.tc + (size_t)inst * n;
-  const double *tPg = (a.tP && S.nnzP > 0) ? a.tP + (size_t)inst * S.nnzP : nullptr;
+  const double *tAg = a.tA + (size_t)inst * a.sA, *tbg = a.tb + (size_t)inst * m, *tcg = a.tc + (size_t)inst * n;
+  const double *tPg = (a.tP && S.nnzP > 0) ? a.tP + (size_t)inst * a.sP : nullptr;
   for (int j = t; j < n; j += T) { M.U[j] = -tcg[j]; M.W[j] = 0.0; }
   __syncthreads();
   AT_mul<DENSE>(S, tAg, M.piy, M.part, [&](int j, double v) { M.U[j] -= v; }, plA);
@@ -292,7 +292,7 @@ template <bool DENSE>
 __device__ __noinline__ void jvp_inactive_rows(const BwdArgs &a, const BwdSmem &M, int inst) {
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, lo = S.z, hi = S.z + S.l;
-  const double *tAg = a.tA + (size_t)inst * S.nnzA, *tbg = a.tb + (size_t)inst * m;
+  const double *tAg = a.tA + (size_t)inst * a.sA, *tbg = a.tb + (size_t)inst * m;
   const double zt = M.X[n + m];
   auto inactive = [&](int i) { return i >= lo && i < hi && !(M.piy[i] > 0); };
   A_mul<DENSE>(S, M.Av, M.X, [&](int i, double v) { if (inactive(i)) M.t1[i] = v - M.b[i] * zt; });
@@ -326,8 +326,8 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
     __syncthreads();
     const int inst = M.ibuf[0];
     if (inst >= a.B) break;
-    const double *Ag = a.A_vals + (size_t)inst * S.nnzA;
-    const double *Pglob = (a.P_vals && S.nnzP > 0) ? a.P_vals + (size_t)inst * S.nnzP : nullptr;
+    const double *Ag = a.A_vals + (size_t)inst * a.sA;
+    const double *Pglob = (a.P_vals && S.nnzP > 0) ? a.P_vals + (size_t)inst * a.sP : nullptr;
     const double *Pg = (Pglob && a.p_in_smem) ? M.Pv : Pglob;
     const bool tmaP = a.use_tma && Pglob && a.p_in_smem && (S.nnzP % 2 == 0) && (((uintptr_t)Pglob & 15) == 0);
     if constexpr (VG) {
@@ -470,7 +470,10 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
       block_reduce<1, false>(r1, M.red);
       const double bnorm = sqrt(r1[0]);
       double beta = bnorm, alfa = 0;
-      for (int k = t; k < N; k += T) { M.U[k] /= beta; M.V[k] = 0.0; }
+      // (beta = 0: the right-hand side vanished under the equilibration -- a forward-mode tangent that lives only in the
+      //  dropped rows of inactive nonneg constraints.  As in SciPy's LSQR the solution is then 0; jvp_inactive_rows recovers
+      //  those rows' unknowns from their own equations.  Dividing by it here turned the whole tangent into NaN.)
+      for (int k = t; k < N; k += T) { M.U[k] = beta > 0 ? M.U[k] / beta : 0.0; M.V[k] = 0.0; }
       acc_BT(M.U, M.V);  // v = B' u
       r1[0] = 0;
       for (int k = t; k < N; k += T) r1[0] = fma(M.V[k], M.V[k], r1[0]);
@@ -552,7 +555,9 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
     {
       const double rt = M.X[N - 1];
       double *dAo = a.dA + (size_t)inst * S.nnzA;
-      if (DENSE) {
+      if (a.srec) {   // shared matrices: r and pi_y for the batch-summing reduction (shared.cu)
+        put_srec(a.srec + (size_t)inst * bc_srec_doubles(n, m), M.X, M.X + n, rt, M.piy, n, m);
+      } else if (DENSE) {
         for (int k = t; k < S.nnzA; k += T) { const int i = k / n, j = k % n; dAo[k] = M.x[j] * M.X[n + i] - M.piy[i] * M.X[j]; }
       } else {
         for (int k = t; k < S.nnzA; k += T) {
@@ -562,7 +567,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
       }
       for (int i = t; i < m; i += T) a.db[(size_t)inst * m + i] = M.piy[i] * rt - M.X[n + i];
       for (int j = t; j < n; j += T) a.dc[(size_t)inst * n + j] = M.x[j] * rt - M.X[j];
-      if (a.dP && S.nnzP > 0) {
+      if (a.dP && S.nnzP > 0 && !a.srec) {
         double *dPo = a.dP + (size_t)inst * S.nnzP;
         for (int k = t; k < S.nnzP; k += T) {
           const int i = __ldg(S.P_rowof + k), j = __ldg(S.P_indices + k);

@@ -62,8 +62,8 @@ __global__ void __launch_bounds__(512, 1) bwd_block_kernel(const __grid_constant
     __syncthreads();
     const int inst = M.ibuf[0];
     if (inst >= a.B) break;
-    const double *Ag = a.A_vals + (size_t)inst * S.nnzA;
-    const double *Pg = a.P_vals + (size_t)inst * S.nnzP;
+    const double *Ag = a.A_vals + (size_t)inst * a.sA;
+    const double *Pg = a.P_vals + (size_t)inst * a.sP;
     const double *dxg = a.dx + (size_t)inst * n, *dyg = a.dy + (size_t)inst * m;
     PhaseTimer pt; pt.start(a.prof);
     // ---- vectors, pi_y, dz ----
@@ -328,13 +328,17 @@ __global__ void __launch_bounds__(512, 1) bwd_block_kernel(const __grid_constant
     // ---- gradient assembly on every structural entry (SURVEY.md 8a B4) ----
     {
       double *dAo = a.dA + (size_t)inst * S.nnzA;
-      for (int k = t; k < S.nnzA; k += T) {
-        const int i = k / n, j = k - i * n;
-        dAo[k] = M.x[j] * M.ry[i] - M.piy[i] * M.t2[j];
+      if (a.srec) {   // shared matrices: r and pi_y for the batch-summing reduction (shared.cu)
+        put_srec(a.srec + (size_t)inst * bc_srec_doubles(n, m), M.t2, M.ry, rt, M.piy, n, m);
+      } else {
+        for (int k = t; k < S.nnzA; k += T) {
+          const int i = k / n, j = k - i * n;
+          dAo[k] = M.x[j] * M.ry[i] - M.piy[i] * M.t2[j];
+        }
       }
       for (int i = t; i < m; i += T) a.db[(size_t)inst * m + i] = M.piy[i] * rt - M.ry[i];
       for (int j = t; j < n; j += T) a.dc[(size_t)inst * n + j] = M.x[j] * rt - M.t2[j];
-      if (a.dP) {
+      if (a.dP && !a.srec) {
         double *dPo = a.dP + (size_t)inst * S.nnzP;
         for (int k = t; k < S.nnzP; k += T) {
           const int i = __ldg(S.P_rowof + k), j = __ldg(S.P_indices + k);

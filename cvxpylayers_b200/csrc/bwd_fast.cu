@@ -207,8 +207,8 @@ __global__ void __launch_bounds__(512, 1) bwd_fast_kernel(const __grid_constant_
     __syncthreads();
     const int inst = M.ibuf[0];
     if (inst < 0) break;
-    const double *Ag = a.A_vals + (size_t)inst * S.nnzA;
-    const double *Pglob = hasP ? a.P_vals + (size_t)inst * S.nnzP : nullptr;
+    const double *Ag = a.A_vals + (size_t)inst * a.sA;
+    const double *Pglob = hasP ? a.P_vals + (size_t)inst * a.sP : nullptr;
     const bool tmaP = a.use_tma && hasP && (S.nnzP % 2 == 0) && (((uintptr_t)a.P_vals & 15) == 0);   // bulk copies need 16-byte aligned sources
     if (a.use_tma) {
       if (t == 0) {
@@ -404,13 +404,17 @@ __global__ void __launch_bounds__(512, 1) bwd_fast_kernel(const __grid_constant_
     {
       const double rt = M.X[N - 1];
       double *dAo = a.dA + (size_t)inst * S.nnzA;
-      for (int k = t; k < S.nnzA; k += T) {   // coalesced stores along the row-major CSR order
-        const int i = k / n, j = k - i * n;
-        dAo[k] = M.x[j] * M.X[n + i] - M.piy[i] * M.X[j];
+      if (a.srec) {   // shared matrices: r and pi_y for the batch-summing reduction (shared.cu)
+        put_srec(a.srec + (size_t)inst * bc_srec_doubles(n, m), M.X, M.X + n, rt, M.piy, n, m);
+      } else {
+        for (int k = t; k < S.nnzA; k += T) {   // coalesced stores along the row-major CSR order
+          const int i = k / n, j = k - i * n;
+          dAo[k] = M.x[j] * M.X[n + i] - M.piy[i] * M.X[j];
+        }
       }
       for (int i = t; i < m; i += T) a.db[(size_t)inst * m + i] = M.piy[i] * rt - M.X[n + i];
       for (int j = t; j < n; j += T) a.dc[(size_t)inst * n + j] = M.x[j] * rt - M.X[j];
-      if (a.dP && hasP) {
+      if (a.dP && hasP && !a.srec) {
         double *dPo = a.dP + (size_t)inst * S.nnzP;
         for (int k = t; k < S.nnzP; k += T) {
           const int i = __ldg(S.P_rowof + k), j = __ldg(S.P_indices + k);

@@ -62,6 +62,10 @@ struct FwdArgs {
   int cache_reuse;       // 0: write the set-up of this solve; 1: A and P are unchanged since the solve that wrote it -> skip it
   int slab_vectors;      // values-off-chip build (fwd_kernel<.., VG = true>): the vectors (and a direct solve's factor) follow the
                          // values in the slab; 0 = they stay in shared memory
+  // batch stride (doubles) of A_vals / P_vals: nnzA / nnzP, or 0 when one copy is shared by the batch (bcone_solve_shared).
+  // cache_stride = 0 likewise marks a set-up record shared by the batch: read only, an instance that re-scales re-factorises
+  // privately and leaves the record alone (other CTAs are reading it).
+  long long sA, sP;
 };
 
 struct BwdArgs {
@@ -85,7 +89,21 @@ struct BwdArgs {
   // tangents of the solution out (ts may be NULL).  Unused by the adjoint kernels.
   const double *tA, *tP, *tb, *tc;
   double *tx, *ty, *ts;
+  // batch stride (doubles) of A_vals / P_vals and of the tangents tA / tP: nnzA / nnzP, or 0 = one copy shared by the batch
+  long long sA, sP;
+  // shared matrices (bcone_vjp_shared): instead of dA / dP, each instance writes r and pi_y here (bc_srec_doubles apart,
+  // layout at put_srec) for the batch-summing reduction of shared.cu.  NULL = assemble dA / dP per instance.
+  double *srec;
 };
+
+// Per-instance record of the shared-matrix adjoint: [r_x n | r_y m | r_tau | pi_y m].
+__host__ __device__ inline long long bc_srec_doubles(int n, int m) { return (long long)n + 2LL * m + 1; }
+// Written by the whole block; rx / ry / piy in shared memory (rx and ry may be one vector X = [r_x ; r_y ; r_tau]).
+static __device__ __noinline__ void put_srec(double *rec, const double *rx, const double *ry, double rt, const double *piy, int n, int m) {
+  for (int j = threadIdx.x; j < n; j += blockDim.x) rec[j] = rx[j];
+  for (int i = threadIdx.x; i < m; i += blockDim.x) { rec[n + i] = ry[i]; rec[n + m + 1 + i] = piy[i]; }
+  if (threadIdx.x == 0) rec[n + m] = rt;
+}
 
 // Phase timing (debug): thread 0 of every CTA adds the cycles since the previous stamp to prof[phase].
 struct PhaseTimer {

@@ -292,8 +292,8 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) fwd_kernel(c
     __syncthreads();
     const int inst = M.ibuf[0];
     if (inst >= a.B) break;
-    const double *Ag = a.A_vals + (size_t)inst * S.nnzA;
-    const double *Pg = (a.P_vals && S.nnzP > 0) ? a.P_vals + (size_t)inst * S.nnzP : nullptr;
+    const double *Ag = a.A_vals + (size_t)inst * a.sA;
+    const double *Pg = (a.P_vals && S.nnzP > 0) ? a.P_vals + (size_t)inst * a.sP : nullptr;
     const double *bg = a.b + (size_t)inst * m, *cg = a.c + (size_t)inst * n;
     PhaseTimer pt; pt.start(a.prof);
     SUB_DECL(pi);

@@ -612,14 +612,14 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
       if (k < a.B && a.cache) {
         double *hd = a.cache + (size_t)k * a.cache_stride;
         ru = a.cache_reuse && hd[1] == 1.0 && hd[2] == a.st.rho_x;
-        if (!ru) hd[1] = 0.0;
+        if (!ru && a.cache_stride) hd[1] = 0.0;   // (a shared record, cache_stride = 0, is never written by the batch)
       }
       ibuf[3] = ru;
     }
     __syncthreads();
     const int inst = ibuf[0];
     if (inst >= a.B) break;
-    const double *Pg = (a.P_vals && S.nnzP > 0) ? a.P_vals + (size_t)inst * S.nnzP : nullptr;
+    const double *Pg = (a.P_vals && S.nnzP > 0) ? a.P_vals + (size_t)inst * a.sP : nullptr;
     long long *pt_t0 = reinterpret_cast<long long *>(sc + SC_COUNT);
     if (a.prof && t == 0) *pt_t0 = clock64();
     auto pt_stamp = [&](int k) { if (a.prof && t == 0) { const long long now = clock64(); atomicAdd(a.prof + k, (unsigned long long)(now - *pt_t0)); *pt_t0 = now; } };
@@ -627,7 +627,7 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
 
     // ---- stage the instance ----
     {
-      const double *Ag = a.A_vals + (size_t)inst * S.nnzA;
+      const double *Ag = a.A_vals + (size_t)inst * a.sA;
       if (a.use_tma) {
         if (t == 0) {
           fence_proxy_async();
@@ -753,7 +753,7 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
         }
       }
     }
-    if (a.cache && !ibuf[3]) cache_vectors<true>(a.cache + (size_t)inst * a.cache_stride + g.cE(), vx(VX_EN), n, g.npad(), vy(VY_DM), m);
+    if (a.cache && a.cache_stride && !ibuf[3]) cache_vectors<true>(a.cache + (size_t)inst * a.cache_stride + g.cE(), vx(VX_EN), n, g.npad(), vy(VY_DM), m);
     {
       double v[2] = {0, 0};
       if (t < m) { const double q = vy(VY_DM)[t] * vy(VY_BH)[t]; vy(VY_BH)[t] = q; v[0] = fabs(q); }
@@ -832,7 +832,7 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
         load_tile();
         __syncthreads();
         form_Kinv(Li, n, g.npad(), g.kst(), Kinv);
-        if (rec) cache_put_kinv(rec, g.cK(), Kinv, (n * g.kst()) >> 1, scale, st.rho_x);
+        if (rec && a.cache_stride) cache_put_kinv(rec, g.cK(), Kinv, (n * g.kst()) >> 1, scale, st.rho_x);   // (shared record: private re-factorisation)
         }
         {   // asynchronous loads behind one barrier phase: P in CSR order into the factor's buffer (for the termination
             // checks) and, with a cached set-up, Kinv

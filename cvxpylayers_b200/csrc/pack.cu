@@ -85,10 +85,11 @@ __global__ void __launch_bounds__(256) e2b_kernel(const double *__restrict__ in,
 // once.  p2e_kernel evaluates the map straight into the engine's instance-contiguous tiles: same tile geometry as
 // b2e_kernel, but a tile row is sum_e val_e p_stack[col_e, i] over the CSR row of the parameter matrix (lanes along the
 // batch axis: every p_stack read is coalesced) instead of a copy.
-//   out[i * ldo + dmap(k)] = sign * sum_{e in row (roff + smap(k))} val[e] * p[col[e] * B + i]
+//   out[i * ldo + dmap(k)] = sign * sum_{e in row (roff + smap(k))} val[e] * p[col[e] * ldp + i]
+// (ldp: row pitch of p_stack -- B, or the full batch when only its first columns are read, as for shared matrices)
 __global__ void __launch_bounds__(256) p2e_kernel(const double *__restrict__ p, const int *__restrict__ rptr, const int *__restrict__ cols,
                                                   const double *__restrict__ vals, double *__restrict__ out, int K, int B, int ldo, int roff,
-                                                  const int *__restrict__ smap, const int *__restrict__ dmap, double sign) {
+                                                  const int *__restrict__ smap, const int *__restrict__ dmap, double sign, long long ldp) {
   __shared__ double tile[TK][TI + 1];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int k0 = blockIdx.x * TK, i0 = blockIdx.y * TI;
@@ -101,7 +102,7 @@ __global__ void __launch_bounds__(256) p2e_kernel(const double *__restrict__ p, 
     double a0 = 0.0, a1 = 0.0;
     for (int e = e0; e < e1; e++) {
       const double v = __ldg(vals + e);
-      const double *col = p + (size_t)(__ldg(cols + e) & 0x3fffffff) * B;   // (bit 30: exclusive-column flag of the way back)
+      const double *col = p + (size_t)(__ldg(cols + e) & 0x3fffffff) * ldp;   // (bit 30: exclusive-column flag of the way back)
       if (i < B) a0 = fma(v, col[i], a0);
       if (i + 32 < B) a1 = fma(v, col[i + 32], a1);
     }
@@ -117,14 +118,14 @@ __global__ void __launch_bounds__(256) p2e_kernel(const double *__restrict__ p, 
     }
   }
 }
-// Transposed map on the way back: dp[col, i] += sign * val[e] * in[i * ldi + smap(k)] for every entry e of row
+// Transposed map on the way back: dp[col * ldp + i] += sign * val[e] * in[i * ldi + smap(k)] for every entry e of row
 // (roff + dmap(k)) of the parameter matrix.  One pass over the engine-layout gradient (tile transposed through shared
 // memory exactly like e2b_kernel), then lanes along the batch axis update dp: entries flagged exclusive (the only entry
 // of their parameter column, the usual "this matrix entry IS a parameter" case; flag = bit 30 of col) are plain stores,
 // the others are fp64 atomic adds (dp is zeroed by the caller).  Column `skip` (the constant 1 row of p_stack) is dropped.
 __global__ void __launch_bounds__(256) e2p_kernel(const double *__restrict__ in, const int *__restrict__ rptr, const int *__restrict__ cols,
                                                   const double *__restrict__ vals, double *__restrict__ dp, int K, int B, int ldi, int roff,
-                                                  const int *__restrict__ smap, const int *__restrict__ dmap, double sign, int skip) {
+                                                  const int *__restrict__ smap, const int *__restrict__ dmap, double sign, int skip, long long ldp) {
   __shared__ double tile[TK][TI + 1];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int k0 = blockIdx.x * TK, i0 = blockIdx.y * TI;
@@ -146,7 +147,7 @@ __global__ void __launch_bounds__(256) e2p_kernel(const double *__restrict__ in,
       const int cf = __ldg(cols + e), c = cf & 0x3fffffff;
       if (c == skip) continue;
       const double v = sign * __ldg(vals + e);
-      double *row = dp + (size_t)c * B + i0;
+      double *row = dp + (size_t)c * ldp + i0;
       if (cf & 0x40000000) {
         if (i0 + tx < B) row[tx] = v * tile[kk][tx];
         if (i0 + tx + 32 < B) row[tx + 32] = v * tile[kk][tx + 32];
@@ -242,17 +243,17 @@ extern "C" cudaError_t bc_scatter_cols(const double *gout, const double *out, lo
 }
 
 extern "C" cudaError_t bc_p2e(const double *p, const int *rptr, const int *cols, const double *vals, double *out, int K, int B, int ldo, int roff,
-                              const int *smap, const int *dmap, double sign, cudaStream_t st) {
+                              const int *smap, const int *dmap, double sign, long long ldp, cudaStream_t st) {
   if (K <= 0 || B <= 0) return cudaSuccess;
   dim3 grid((K + TK - 1) / TK, (B + TI - 1) / TI);
-  p2e_kernel<<<grid, 256, 0, st>>>(p, rptr, cols, vals, out, K, B, ldo, roff, smap, dmap, sign);
+  p2e_kernel<<<grid, 256, 0, st>>>(p, rptr, cols, vals, out, K, B, ldo, roff, smap, dmap, sign, ldp);
   return cudaGetLastError();
 }
 extern "C" cudaError_t bc_e2p(const double *in, const int *rptr, const int *cols, const double *vals, double *dp, int K, int B, int ldi, int roff,
-                              const int *smap, const int *dmap, double sign, int skip, cudaStream_t st) {
+                              const int *smap, const int *dmap, double sign, int skip, long long ldp, cudaStream_t st) {
   if (K <= 0 || B <= 0) return cudaSuccess;
   dim3 grid((K + TK - 1) / TK, (B + TI - 1) / TI);
-  e2p_kernel<<<grid, 256, 0, st>>>(in, rptr, cols, vals, dp, K, B, ldi, roff, smap, dmap, sign, skip);
+  e2p_kernel<<<grid, 256, 0, st>>>(in, rptr, cols, vals, dp, K, B, ldi, roff, smap, dmap, sign, skip, ldp);
   return cudaGetLastError();
 }
 

@@ -26,7 +26,7 @@ _ARG_MAP = {
     "lsqr_iter_lim": "lsqr_iter_lim", "lsqr_precond": "lsqr_precond", "adaptive_check": "adaptive_check",
     "acceleration_lookback": "acceleration_lookback", "acceleration_interval": "acceleration_interval",
 }
-_IGNORED = {"verbose", "n_jobs_forward", "n_jobs_backward", "solve_method", "warm_starts", "raise_on_error", "warm_start", "reuse_setup"}   # (warm_start / reuse_setup are handled by the layer)
+_IGNORED = {"verbose", "n_jobs_forward", "n_jobs_backward", "solve_method", "warm_starts", "raise_on_error", "warm_start", "reuse_setup", "shared_matrices"}   # (warm_start / reuse_setup / shared_matrices are handled by the layer)
 
 
 def make_settings(args: dict | None) -> _lib.BconeSettings:
@@ -265,28 +265,35 @@ class Engine:
         self._raise(rc, "bcone_set_param_maps")
         self._P1 = P1
 
-    def ingest_params(self, p_stack: torch.Tensor, out=None):
-        """p_stack[P1, B] -> engine-layout (A_vals, P_vals, b, c) without materialising A_eval."""
+    def ingest_params(self, p_stack: torch.Tensor, out=None, shared: bool = False):
+        """p_stack[P1, B] -> engine-layout (A_vals, P_vals, b, c) without materialising A_eval.
+        ``shared=True``: A_vals[nnzA] / P_vals[nnzP] are evaluated once, from column 0 (the parameters feeding A and P are
+        unbatched); b and c from every column."""
         st, dev, f64 = self.structure, self.device, torch.float64
         B = p_stack.shape[1]
         _chk(p_stack, (self._P1, B), f64, dev, "p_stack")
         if out is not None:
             A_vals, P_vals, b, c = out
         else:
-            A_vals = torch.empty((B, st.nnzA), dtype=f64, device=dev)
+            lead = () if shared else (B,)
+            A_vals = torch.empty((*lead, st.nnzA), dtype=f64, device=dev)
             b = torch.empty((B, st.m), dtype=f64, device=dev)
             c = torch.empty((B, st.n), dtype=f64, device=dev)
-            P_vals = torch.empty((B, st.nnzP), dtype=f64, device=dev) if st.nnzP else None
-        rc = self.lib.bcone_ingest_params(self.h, C.c_int32(B), _ptr(p_stack), _ptr(A_vals), _ptr(P_vals), _ptr(b), _ptr(c), self._stream())
-        self._raise(rc, "bcone_ingest_params")
+            P_vals = torch.empty((*lead, st.nnzP), dtype=f64, device=dev) if st.nnzP else None
+        fn = self.lib.bcone_ingest_params_shared if shared else self.lib.bcone_ingest_params
+        rc = fn(self.h, C.c_int32(B), _ptr(p_stack), _ptr(A_vals), _ptr(P_vals), _ptr(b), _ptr(c), self._stream())
+        self._raise(rc, "bcone_ingest_params_shared" if shared else "bcone_ingest_params")
         return A_vals, P_vals, b, c
 
-    def emit_params(self, dA_vals, dP_vals, db, dc, out=None):
-        """engine gradients -> dp_stack[P1, B] (transposed parameter maps; the constant's row stays 0)."""
-        B = dA_vals.shape[0]
+    def emit_params(self, dA_vals, dP_vals, db, dc, out=None, shared: bool = False):
+        """engine gradients -> dp_stack[P1, B] (transposed parameter maps; the constant's row stays 0).
+        ``shared=True``: dA_vals[nnzA] / dP_vals[nnzP] are batch sums (:meth:`vjp` on shared matrices); their contribution goes
+        into column 0, that of db / dc into every column."""
+        B = db.shape[0]
         dp = out if out is not None else torch.empty((self._P1, B), dtype=torch.float64, device=self.device)
-        rc = self.lib.bcone_emit_params(self.h, C.c_int32(B), _ptr(dA_vals), _ptr(dP_vals), _ptr(db), _ptr(dc), _ptr(dp), self._stream())
-        self._raise(rc, "bcone_emit_params")
+        fn = self.lib.bcone_emit_params_shared if shared else self.lib.bcone_emit_params
+        rc = fn(self.h, C.c_int32(B), _ptr(dA_vals), _ptr(dP_vals), _ptr(db), _ptr(dc), _ptr(dp), self._stream())
+        self._raise(rc, "bcone_emit_params_shared" if shared else "bcone_emit_params")
         return dp
 
     # ------------------------------------------------------------------ forward / backward
@@ -302,16 +309,21 @@ class Engine:
     def solve(self, A_vals, b, c, P_vals=None, settings: _lib.BconeSettings | None = None, out: "Solution | None" = None,
               warm: "tuple | Solution | None" = None, cache=None, reuse: bool = False) -> Solution:
         """``cache`` (from :meth:`new_cache`): keep the equilibration and the factorisation of every instance; ``reuse=True``
-        states that ``A_vals`` / ``P_vals`` are those of the call that filled it (``b`` and ``c`` may differ) and skips them."""
+        states that ``A_vals`` / ``P_vals`` are those of the call that filled it (``b`` and ``c`` may differ) and skips them.
+        1-D ``A_vals[nnzA]`` (and ``P_vals[nnzP]``): one copy shared by the batch (``bcone_solve_shared``; B from ``b``)."""
         st, dev, f64 = self.structure, self.device, torch.float64
-        B = A_vals.shape[0]
-        _chk(A_vals, (B, st.nnzA), f64, dev, "A_vals")
+        shared = A_vals.dim() == 1
+        B = b.shape[0] if shared else A_vals.shape[0]
+        lead = () if shared else (B,)
+        _chk(A_vals, (*lead, st.nnzA), f64, dev, "A_vals")
         _chk(b, (B, st.m), f64, dev, "b")
         _chk(c, (B, st.n), f64, dev, "c")
         if st.nnzP:
             if P_vals is None:
                 raise ValueError("structure has a quadratic term but P_vals is None")
-            _chk(P_vals, (B, st.nnzP), f64, dev, "P_vals")
+            _chk(P_vals, (*lead, st.nnzP), f64, dev, "P_vals")
+        if shared and cache is not None:
+            raise ValueError("cache: a shared-matrix solve keeps its own set-up (pass cache=None)")
         settings = settings or _lib.default_settings()
         if out is not None:
             x, y, s, status, iters, resid = out.x, out.y, out.s, out.status, out.iters, out.resid
@@ -329,50 +341,65 @@ class Engine:
                 _chk(t_, shp, f64, dev, name)
         if cache is not None and (cache.dtype != f64 or cache.device != dev or cache.numel() * 8 < self.cache_bytes(B) or not cache.is_contiguous()):
             raise ValueError("cache: need a contiguous float64 tensor of cache_bytes(B) bytes on the engine's device (engine.new_cache(B))")
-        rc = self.lib.bcone_solve_cached(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c),
-                                         _ptr(x0), _ptr(y0), _ptr(s0), _ptr(x), _ptr(y), _ptr(s), _ptr(status), _ptr(iters), _ptr(resid),
-                                         _ptr(cache), C.c_int32(1 if (cache is not None and reuse) else 0), C.byref(settings), self._stream())
-        self._raise(rc, "bcone_solve")
+        if shared:
+            rc = self.lib.bcone_solve_shared(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c),
+                                             _ptr(x0), _ptr(y0), _ptr(s0), _ptr(x), _ptr(y), _ptr(s), _ptr(status), _ptr(iters), _ptr(resid),
+                                             C.byref(settings), self._stream())
+        else:
+            rc = self.lib.bcone_solve_cached(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c),
+                                             _ptr(x0), _ptr(y0), _ptr(s0), _ptr(x), _ptr(y), _ptr(s), _ptr(status), _ptr(iters), _ptr(resid),
+                                             _ptr(cache), C.c_int32(1 if (cache is not None and reuse) else 0), C.byref(settings), self._stream())
+        self._raise(rc, "bcone_solve_shared" if shared else "bcone_solve")
         return Solution(x, y, s, status, iters, resid)
 
     def vjp(self, A_vals, b, c, x, y, s, dx, dy, P_vals=None, settings: _lib.BconeSettings | None = None, out=None):
-        """-> dA_vals[B,nnzA], dP_vals[B,nnzP]|None, db[B,m], dc[B,n], lsqr_iters[B]  (``out``: the same five, preallocated)"""
+        """-> dA_vals[B,nnzA], dP_vals[B,nnzP]|None, db[B,m], dc[B,n], lsqr_iters[B]  (``out``: the same five, preallocated).
+        1-D ``A_vals[nnzA]`` / ``P_vals[nnzP]`` (shared by the batch): dA_vals[nnzA] / dP_vals[nnzP] are the batch sums
+        (``bcone_vjp_shared``)."""
         st, dev, f64 = self.structure, self.device, torch.float64
-        B = A_vals.shape[0]
-        for name, t, shp in (("A_vals", A_vals, (B, st.nnzA)), ("b", b, (B, st.m)), ("c", c, (B, st.n)),
+        shared = A_vals.dim() == 1
+        B = b.shape[0] if shared else A_vals.shape[0]
+        lead = () if shared else (B,)
+        for name, t, shp in (("A_vals", A_vals, (*lead, st.nnzA)), ("b", b, (B, st.m)), ("c", c, (B, st.n)),
                              ("x", x, (B, st.n)), ("y", y, (B, st.m)), ("s", s, (B, st.m)),
                              ("dx", dx, (B, st.n)), ("dy", dy, (B, st.m))):
             _chk(t, shp, f64, dev, name)
+        if shared and st.nnzP:
+            _chk(P_vals, (st.nnzP,), f64, dev, "P_vals")
         settings = settings or _lib.default_settings()
         if out is not None:
             dA, dP, db, dc, its = out
         else:
-            dA = torch.empty((B, st.nnzA), dtype=f64, device=dev)
+            dA = torch.empty((*lead, st.nnzA), dtype=f64, device=dev)
             db = torch.empty((B, st.m), dtype=f64, device=dev)
             dc = torch.empty((B, st.n), dtype=f64, device=dev)
-            dP = torch.empty((B, st.nnzP), dtype=f64, device=dev) if st.nnzP else None
+            dP = torch.empty((*lead, st.nnzP), dtype=f64, device=dev) if st.nnzP else None
             its = torch.empty(B, dtype=torch.int32, device=dev)
-        rc = self.lib.bcone_vjp(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c),
-                                _ptr(x), _ptr(y), _ptr(s), _ptr(dx), _ptr(dy), _ptr(dA), _ptr(dP), _ptr(db), _ptr(dc),
-                                _ptr(its), C.byref(settings), self._stream())
-        self._raise(rc, "bcone_vjp")
+        fn = self.lib.bcone_vjp_shared if shared else self.lib.bcone_vjp
+        rc = fn(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c),
+                _ptr(x), _ptr(y), _ptr(s), _ptr(dx), _ptr(dy), _ptr(dA), _ptr(dP), _ptr(db), _ptr(dc),
+                _ptr(its), C.byref(settings), self._stream())
+        self._raise(rc, "bcone_vjp_shared" if shared else "bcone_vjp")
         return dA, dP, db, dc, its
 
     def jvp(self, A_vals, b, c, x, y, s, dA, db, dc, P_vals=None, dP=None, settings: _lib.BconeSettings | None = None, out=None):
         """Forward-mode derivative of the solution map at (x, y, s) (diffcp's ``D``; the transpose of :meth:`vjp`): tangents of
         the data in engine layout -> dx[B,n], dy[B,m], ds[B,m], lsqr_iters[B]  (``out``: the same four, preallocated).
-        ``dP`` None = no tangent on P."""
+        ``dP`` None = no tangent on P.  1-D ``A_vals`` / ``P_vals`` with 1-D tangents ``dA`` / ``dP``: matrices and their
+        tangents shared by the batch (``bcone_jvp_shared``)."""
         st, dev, f64 = self.structure, self.device, torch.float64
-        B = A_vals.shape[0]
-        for name, t, shp in (("A_vals", A_vals, (B, st.nnzA)), ("b", b, (B, st.m)), ("c", c, (B, st.n)),
+        shared = A_vals.dim() == 1
+        B = b.shape[0] if shared else A_vals.shape[0]
+        lead = () if shared else (B,)
+        for name, t, shp in (("A_vals", A_vals, (*lead, st.nnzA)), ("b", b, (B, st.m)), ("c", c, (B, st.n)),
                              ("x", x, (B, st.n)), ("y", y, (B, st.m)), ("s", s, (B, st.m)),
-                             ("dA", dA, (B, st.nnzA)), ("db", db, (B, st.m)), ("dc", dc, (B, st.n))):
+                             ("dA", dA, (*lead, st.nnzA)), ("db", db, (B, st.m)), ("dc", dc, (B, st.n))):
             _chk(t, shp, f64, dev, name)
         if st.nnzP:
             if P_vals is None:
                 raise ValueError("structure has a quadratic term but P_vals is None")
-            _chk(P_vals, (B, st.nnzP), f64, dev, "P_vals")
-            _chk(dP, (B, st.nnzP), f64, dev, "dP")
+            _chk(P_vals, (*lead, st.nnzP), f64, dev, "P_vals")
+            _chk(dP, (*lead, st.nnzP), f64, dev, "dP")
         settings = settings or _lib.default_settings()
         if out is not None:
             dx, dy, ds, its = out
@@ -381,8 +408,9 @@ class Engine:
             dy = torch.empty((B, st.m), dtype=f64, device=dev)
             ds = torch.empty((B, st.m), dtype=f64, device=dev)
             its = torch.empty(B, dtype=torch.int32, device=dev)
-        rc = self.lib.bcone_jvp(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c),
-                                _ptr(x), _ptr(y), _ptr(s), _ptr(dA), _ptr(dP if st.nnzP else None), _ptr(db), _ptr(dc),
-                                _ptr(dx), _ptr(dy), _ptr(ds), _ptr(its), C.byref(settings), self._stream())
-        self._raise(rc, "bcone_jvp")
+        fn = self.lib.bcone_jvp_shared if shared else self.lib.bcone_jvp
+        rc = fn(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c),
+                _ptr(x), _ptr(y), _ptr(s), _ptr(dA), _ptr(dP if st.nnzP else None), _ptr(db), _ptr(dc),
+                _ptr(dx), _ptr(dy), _ptr(ds), _ptr(its), C.byref(settings), self._stream())
+        self._raise(rc, "bcone_jvp_shared" if shared else "bcone_jvp")
         return dx, dy, ds, its

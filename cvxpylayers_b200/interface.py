@@ -172,6 +172,10 @@ class B200_ctx:
         """The set-up cache of (device, batch size) when the option ``reuse_setup`` is on -- explicitly (the caller states that
         A and P are the same on every call), or by default when the parameter maps show it (``PA_is_constant``) -- else None.
         The engine validates every record itself, so a fresh (zero-filled) cache is simply filled by its first solve."""
+        if merged.get("shared_matrices"):
+            if merged.get("reuse_setup"):
+                raise ValueError("shared_matrices and reuse_setup exclude each other: a shared-matrix solve builds one set-up per call")
+            return None   # (nor the automatic PA_is_constant cache: the batch shares one set-up per call instead)
         if not merged.get("reuse_setup", getattr(self, "PA_is_constant", False)):
             return None
         if not hasattr(self, "_setup_cache"):
@@ -180,6 +184,27 @@ class B200_ctx:
         if key not in self._setup_cache:
             self._setup_cache[key] = eng.new_cache(B)   # None: this structure has no cached path
         return self._setup_cache[key]
+
+    def check_shared_matrices(self, sizes, batched, col_order) -> None:
+        """With ``shared_matrices`` every parameter whose p_stack rows feed A (the first nnzA rows of the A map) or P must be
+        unbatched: the layer evaluates A and P from the first instance only.  Per user parameter i: ``sizes[i]`` entries,
+        ``batched[i]``, ``col_order[i]`` (the reference's ``user_order_to_col_order``); p_stack holds the parameters' rows in
+        column order (``_flatten_and_batch_params``).  Raises ValueError naming the first batched one."""
+        maps = getattr(self, "_param_maps", None)
+        if maps is None:
+            return
+        A_map, _, P_map = maps
+        nA = A_map.shape[0] - len(self.b_idx)
+        used = set(sp.csr_matrix(A_map)[:nA, :-1].indices.tolist())
+        if P_map is not None:
+            used |= set(sp.csr_matrix(P_map)[:, :-1].indices.tolist())
+        acc = 0
+        for i in sorted(range(len(sizes)), key=lambda i: col_order[i]):
+            rows = range(acc, acc + sizes[i])
+            acc += sizes[i]
+            if batched[i] and any(r in used for r in rows):
+                raise ValueError(f"shared_matrices: parameter {i} feeds A or P but is batched; the matrices must come from "
+                                 "unbatched parameters")
 
     def compute_device(self, t: torch.Tensor) -> torch.device:
         if t.is_cuda:
@@ -594,10 +619,13 @@ class _CvxpyLayerFused(torch.autograd.Function):
         merged = {**ctx.options, **(solver_args or {})}
         settings = make_settings(merged)
         B = ps.shape[1]
+        # shared_matrices: the caller states that A and P are the same for every instance (their parameters are unbatched);
+        # they are evaluated once and the batch shares them through solve, adjoint and forward mode
+        shared = bool(merged.get("shared_matrices"))
         with torch.cuda.device(dev):
-            A_vals, P_vals, b, c = eng.ingest_params(_to_dev(ps, dev))
-            sol = eng.solve(A_vals, b, c, P_vals, settings, warm=ctx.warm_for(dev, B, warm_start, merged),
-                            cache=ctx.setup_cache(eng, dev, B, merged), reuse=True)
+            cache = ctx.setup_cache(eng, dev, B, merged)
+            A_vals, P_vals, b, c = eng.ingest_params(_to_dev(ps, dev), shared=shared)
+            sol = eng.solve(A_vals, b, c, P_vals, settings, warm=ctx.warm_for(dev, B, warm_start, merged), cache=cache, reuse=True)
             status = sol.status.cpu()
         ctx.remember(dev, B, sol, merged, warm_start)
         bad = (status != 1) & (status != 2)
@@ -626,10 +654,10 @@ class _CvxpyLayerFused(torch.autograd.Function):
             raise RuntimeError("backward called on a forward pass run with needs_grad=False")
         eng, settings, A_vals, P_vals, b, c, x, y, s = ctx.saved.items
         dev = eng.device
-        B = A_vals.shape[0]
+        B = b.shape[0]
         with torch.cuda.device(dev):
             dA, dP, db, dc, _ = eng.vjp(A_vals, b, c, x, y, s, _to_dev(dprimal, dev).reshape(B, -1), _to_dev(ddual, dev).reshape(B, -1), P_vals, settings)
-            dp = _to_host_like(eng.emit_params(dA, dP, db, dc), in_device, in_dtype)
+            dp = _to_host_like(eng.emit_params(dA, dP, db, dc, shared=A_vals.dim() == 1), in_device, in_dtype)
             if in_device.type == "cpu":
                 torch.cuda.current_stream(dev).synchronize()
         return (dp.squeeze(1) if unb else dp), None, None, None, None
@@ -642,9 +670,9 @@ class _CvxpyLayerFused(torch.autograd.Function):
             raise RuntimeError("forward-mode AD on a forward pass that kept nothing for it")
         eng, settings, A_vals, P_vals, b, c, x, y, s = ctx.saved.items
         dev = eng.device
-        B = A_vals.shape[0]
+        B = b.shape[0]
         with torch.cuda.device(dev):
-            dA, dP, db, dc = eng.ingest_params(_tangent(tp, eng._P1, B, unb, dev))
+            dA, dP, db, dc = eng.ingest_params(_tangent(tp, eng._P1, B, unb, dev), shared=A_vals.dim() == 1)
             dx, dy, _, _ = eng.jvp(A_vals, b, c, x, y, s, dA, db, dc, P_vals, dP, settings)
             dprimal = _to_host_like(dx, in_device, in_dtype)
             ddual = _to_host_like(dy, in_device, in_dtype)
@@ -718,6 +746,10 @@ def register(canon_solver: str = "DIFFCP", fuse: bool = True) -> None:
                 if getattr(self.ctx, "solver", None) != "B200" or getattr(sctx, "_param_maps", None) is None:
                     return orig_forward(self, *params, solver_args=solver_args, warm_start=warm_start, **kw)
                 batch = self.ctx.validate_params(list(params))
+                if {**sctx.options, **(solver_args or {})}.get("shared_matrices") and hasattr(self.ctx, "batch_sizes"):
+                    bs = self.ctx.batch_sizes
+                    sizes = [int(np.prod(p.shape[1:] if bs[i] else p.shape, dtype=np.int64)) for i, p in enumerate(params)]
+                    sctx.check_shared_matrices(sizes, [bool(v) for v in bs], self.ctx.user_order_to_col_order)
                 on_dev = all(p.is_cuda and p.dtype == torch.float64 for p in params) and hasattr(self.ctx, "batch_sizes")
                 if on_dev:   # prologue as index-map launches (layer_io.py, SURVEY.md 8f.3), GP log folded in
                     from . import layer_io  # noqa: PLC0415

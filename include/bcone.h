@@ -192,6 +192,44 @@ int bcone_jvp(void *handle, int32_t B, const double *A_vals, const double *P_val
               const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters,
               const bcone_settings *st, void *cuda_stream);
 
+/* Batch-shared matrices (OptNet-style layers: A and P are learned weights, every instance brings its own b and c).  The
+ * replicated entry points above take A_vals[B,nnzA] / P_vals[B,nnzP] and return dA[B,nnzA] / dP[B,nnzP], which a layer then
+ * sums over the batch; these take ONE copy of the values and return the batch sums, with the same kernels reading the one copy
+ * (batch stride 0; it stays in L2).  Every structure bcone_create accepts works on them.  Results equal the replicated entry
+ * points' on A_vals.expand(B, nnzA): bit for bit where the solve builds K without atomics, up to their launch-to-launch
+ * variation where it does (generic direct forward with SOC / PSD / exp cones or CSR A).
+ *   bcone_solve_shared: A_vals[nnzA], P_vals[nnzP] or NULL, b[B,m], c[B,n], x0 / y0 / s0 as bcone_solve_warm (all NULL = cold),
+ *     outputs as bcone_solve.  On the register-tiled kernel (bcone_path_info fwd 2) the batch also shares ONE set-up: a one-CTA
+ *     launch equilibrates A and P and factorises K at the initial scale into a record the handle keeps per stream, and every
+ *     instance starts from it (as bcone_solve_cached with reuse = 1).  An instance whose adaptive scale changes
+ *     re-factorises privately.
+ *   bcone_vjp_shared: as bcone_vjp, with A_vals[nnzA], P_vals[nnzP]; dA_sum[nnzA] and dP_sum[nnzP] (or NULL) receive
+ *     sum_b of what bcone_vjp returns for instance b; db[B,m], dc[B,n], lsqr_iters[B] stay per instance.  The kernels write
+ *     r and pi_y per instance (n + 2m + 1 doubles, scratch kept by the handle per stream) and a two-stage reduction with a
+ *     fixed order and no floating-point atomics forms the sums: two calls give identical bits.
+ *   bcone_jvp_shared: as bcone_jvp, with A_vals[nnzA], P_vals[nnzP] and the shared tangents dA[nnzA], dP[nnzP] or NULL;
+ *     db[B,m], dc[B,n] and the outputs per instance.
+ *   bcone_ingest_params_shared: as bcone_ingest_params, but A_vals[nnzA] / P_vals[nnzP] are evaluated from column 0 of
+ *     p_stack[P1,B] only (the parameters feeding A and P are unbatched); b and c from every column.
+ *   bcone_emit_params_shared: as bcone_emit_params from dA_sum[nnzA] / dP_sum[nnzP] (or NULL): their contribution goes into
+ *     column 0 of dp_stack[P1,B], that of db / dc into every column.  By linearity the batch sum of dp_stack over the rows of
+ *     an unbatched parameter equals that of the replicated path, and that sum is all a layer's backward consumes. */
+int bcone_solve_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                       const double *x0, const double *y0, const double *s0, double *x, double *y, double *s,
+                       int32_t *status, int32_t *iters, double *resid, const bcone_settings *st, void *cuda_stream);
+int bcone_vjp_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b,
+                     const double *c, const double *x, const double *y, const double *s, const double *dx,
+                     const double *dy, double *dA_sum, double *dP_sum, double *db, double *dc,
+                     int32_t *lsqr_iters, const bcone_settings *st, void *cuda_stream);
+int bcone_jvp_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                     const double *x, const double *y, const double *s, const double *dA, const double *dP,
+                     const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters,
+                     const bcone_settings *st, void *cuda_stream);
+int bcone_ingest_params_shared(void *handle, int32_t B, const double *p_stack, double *A_vals, double *P_vals, double *b,
+                               double *c, void *cuda_stream);
+int bcone_emit_params_shared(void *handle, int32_t B, const double *dA_sum, const double *dP_sum, const double *db,
+                             const double *dc, double *dp_stack, void *cuda_stream);
+
 /* Pitched host<->device copy on the caller's stream (bytes): moves a batch slice [rows, lo:hi] of a
  * boundary tensor directly between pinned host memory and a contiguous device chunk. */
 int bcone_memcpy2d(void *dst, int64_t dpitch, const void *src, int64_t spitch, int64_t width, int64_t height,
