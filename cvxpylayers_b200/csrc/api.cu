@@ -10,50 +10,47 @@
 #include <cstdlib>
 #include "common.cuh"
 
-// ---- kernels / launchers implemented in fwd.cu, bwd.cu, pack.cu ----
-extern "C" {
-size_t bc_fwd_smem_bytes(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp, int vals_global);
-size_t bc_fwd_ws_doubles(int n, int m, int vectors, int with_factor, int nnzA_global);
-cudaError_t bc_fwd_configure(int dense, int indirect, size_t smem, int small_cta, int vg);
-cudaError_t bc_fwd_occupancy(int dense, int indirect, int threads, size_t smem, int *ctas, int small_cta, int vg);
-cudaError_t bc_fwd_launch(const FwdArgs *a, int indirect, int grid, int threads, size_t smem, cudaStream_t st, int small_cta, int vg);
-size_t bc_fwdf_smem_bytes(int n, int m);
-int bc_fwdf_threads(void);
-size_t bc_fwdf_cache_doubles(int n, int m);
-int bc_fwdf_eligible(int n, int m);
-cudaError_t bc_fwdf_configure(int n, int m, size_t smem);
-cudaError_t bc_fwdf_occupancy(int n, int m, size_t smem, int *ctas);
-cudaError_t bc_fwdf_launch(const FwdArgs *a, int grid, size_t smem, cudaStream_t st);
-size_t bc_bwd_ws_doubles(int n, int m, int npoly);
-size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global, int vals_global);
-cudaError_t bc_bwd_configure(int dense, size_t smem, int small_cta, int vg);
-cudaError_t bc_bwd_occupancy(int dense, int threads, size_t smem, int *ctas, int small_cta, int vg);
-cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st, int small_cta, int vg);
-cudaError_t bc_jvp_configure(int dense, size_t smem, int small_cta, int vg);
-cudaError_t bc_jvp_occupancy(int dense, int threads, size_t smem, int *ctas, int small_cta, int vg);
-cudaError_t bc_jvp_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st, int small_cta, int vg);
-size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads);
-cudaError_t bc_bwdf_configure(int n, size_t smem);
-cudaError_t bc_bwdf_occupancy(int n, int threads, size_t smem, int *ctas);
-cudaError_t bc_bwdf_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st);
-size_t bc_bwdb_smem_bytes(int n, int m, int threads);
-cudaError_t bc_bwdb_configure(size_t smem);
-cudaError_t bc_bwdb_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t st);
-cudaError_t bc_b2e(const double *in, double *out, int K, int B, int ldo, int roff, const int *smap, const int *dmap, double sign, long long ldb, cudaStream_t st);
-cudaError_t bc_e2b(const double *in, double *out, int K, int B, int ldi, int roff, const int *smap, const int *dmap, double sign, long long ldb, cudaStream_t st);
-cudaError_t bc_rows_from_param(const double *param, long long stride, const int *map, int K, int B, int op, double *rows, cudaStream_t st);
-cudaError_t bc_param_from_rows(const double *grows, const double *param, long long stride, const int *map, int K, int B, int op, double *gparam, cudaStream_t st);
-cudaError_t bc_gather_cols(const double *in, long long ld, const int *map, const double *scale, int K, int B, int op, double *out, cudaStream_t st);
-cudaError_t bc_scatter_cols(const double *gout, const double *out, long long ld, const int *map, const double *scale, int K, int B, int op, double *gin, cudaStream_t st);
-cudaError_t bc_p2e(const double *p, const int *rptr, const int *cols, const double *vals, double *out, int K, int B, int ldo, int roff,
-                   const int *smap, const int *dmap, double sign, long long ldp, cudaStream_t st);
-cudaError_t bc_e2p(const double *in, const int *rptr, const int *cols, const double *vals, double *dp, int K, int B, int ldi, int roff,
-                   const int *smap, const int *dmap, double sign, int skip, long long ldp, cudaStream_t st);
-size_t bc_shared_part_doubles(const DevStruct *S, int B);
-cudaError_t bc_shared_grad(const DevStruct *S, const double *rec, const double *x, int B, double *dA, double *dP, double *part, cudaStream_t st);
-}
-
 namespace {
+// One kernel's launch plan: its address (from the bc_*_kernel lookup of its file), block size, dynamic shared memory and the
+// CTAs one SM keeps resident (>= 1 once configured).
+struct Plan { const void *fn = nullptr; int threads = 0; size_t smem = 0; int ctas = 0; };
+cudaError_t configure(Plan &p) {
+  if (!p.fn) return cudaErrorInvalidDeviceFunction;   // no such instantiation
+  const cudaError_t e = cudaFuncSetAttribute(p.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem);
+  if (e != cudaSuccess) return e;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p.ctas, p.fn, p.threads, p.smem) != cudaSuccess || p.ctas < 1) p.ctas = 1;
+  return cudaSuccess;
+}
+// args: the kernel's one argument block (FwdArgs / BwdArgs)
+cudaError_t launch(const Plan &p, int grid, const void *args, cudaStream_t st) {
+  void *argv[] = {const_cast<void *>(args)};
+  cudaLaunchKernel(p.fn, dim3(grid), dim3(p.threads), argv, p.smem, st);
+  return cudaGetLastError();   // (read and cleared: not left for the caller's next CUDA call)
+}
+int grid_for(const Plan &p, int B, int num_sms) { return std::min(B, num_sms * p.ctas); }
+
+// A generic kernel's plan.  <= 256-thread instances have a second build of the generic kernels for four resident CTAs per SM
+// (64 registers).  It wins when the batch exceeds what the 128-register build keeps resident (more CTAs overlap each other's
+// stalls: exp-cone workload) and loses when every instance is resident anyway and only its own latency counts (SDP at B = 256),
+// so the choice is made per launch from the batch size.  BCONE_SMALL_CTA=0 disables, =2 forces.
+struct TieredPlan {
+  Plan big, small;
+  bool has_small = false;
+  int indirect = 0;        // forward, large instances: CG instead of Cholesky, vectors in a global slab
+  int factor_global = 0;   // forward, in between: values on chip, vectors + packed Cholesky factor in the slab (direct solve from L2 / HBM)
+  int p_in_smem = 0, vec_global = 0;   // LSQR: P staged in shared memory; large instances: vectors in a global slab
+  // values off chip (the tier after every on-chip option): the forward copies each instance's CSR values into its CTA's slab,
+  // the backward / forward-mode LSQR reads them in place from A_vals.  Only 512-thread builds exist for it (no small variant).
+  int vals_global = 0;
+  size_t ws_stride = 0;    // doubles of slab per CTA
+};
+// the 4-CTA/SM build only when the batch does not fit the resident capacity of the 128-register build
+const Plan &pick(const TieredPlan &t, int B, int num_sms, int small_mode) {
+  return t.has_small && (small_mode == 2 || B > num_sms * t.big.ctas) ? t.small : t.big;
+}
+// CTAs of the largest grid either build launches: what the per-CTA slabs are sized for
+size_t max_grid(const TieredPlan &t, int num_sms) { return (size_t)num_sms * std::max(t.big.ctas, t.has_small ? t.small.ctas : 0); }
+
 struct Handle {
   DevStruct S{};
   int device = 0, max_batch = 0, num_sms = 0;
@@ -68,17 +65,18 @@ struct Handle {
   struct PMap { int *ptr = nullptr, *col = nullptr; double *val = nullptr; int rows = 0; };
   PMap pmA, pmq, pmP;
   int P1 = 0;
-  int fwd_threads = 0, bwd_threads = 0, fwd_ctas = 0, bwd_ctas = 0;
-  size_t fwd_smem = 0, bwd_smem = 0;
-  int tma_ok = 0, psd_total = 0, p_in_smem = 0;
-  int fwd_indirect = 0, bwd_vec_global = 0;   // large instances: CG instead of Cholesky, vectors in a global slab
-  // <= 256-thread instances have a second build of the generic kernels for four resident CTAs per SM (64 registers).  It wins
-  // when the batch exceeds what the 128-register build keeps resident (more CTAs overlap each other's stalls: exp-cone workload)
-  // and loses when every instance is resident anyway and only its own latency counts (SDP at B = 256), so the
-  // choice is made per launch from the batch size.  BCONE_SMALL_CTA=0 disables, =2 forces.
-  int fwd_small = 0, bwd_small = 0, fwd_ctas_small = 0, bwd_ctas_small = 0, small_mode = 1;
-  int fwd_factor_global = 0;                  // in between: values on chip, vectors + packed Cholesky factor in the slab (direct solve from L2 / HBM)
-  size_t fwd_ws_stride = 0, bwd_ws_stride = 0;
+  int tma_ok = 0, psd_total = 0;
+  // Launch plans, chosen once in bcone_create.  The generic kernels (fwd.cu; bwd.cu as adjoint and as forward mode) each have a
+  // TieredPlan; fast_fwd / fast_bwd / block_bwd say where a specialised kernel runs instead.
+  TieredPlan fwd, bwd;
+  // forward-mode derivative (bcone_jvp): always the generic kernel (bwd.cu, JVP = true), so structures on the fused backward
+  // need a generic geometry of their own; chosen by the same rule as the generic backward's.  jvp_ok = 0: none fits.
+  TieredPlan jvp; int jvp_ok = 0;
+  Plan fwd_fast;    // fast_fwd: dense A, polyhedral cones, direct mode: register-tiled forward (fwd_fast.cu)
+  Plan bwd_fast;    // fast_bwd: dense A, polyhedral cones, dense-or-no P: fused single-pass backward (bwd_fast.cu)
+  Plan bwd_block;   // block_bwd: KKT-block preconditioned backward (lsqr_precond = 2)
+  int fast_fwd = 0, fast_bwd = 0, block_bwd = 0;
+  int small_mode = 1;   // BCONE_SMALL_CTA: 0 disables the 4-CTA/SM builds, 2 forces them
   // Per-stream scratch slabs (one per CTA of the grid): launches on different streams may overlap, launches on one
   // stream cannot, so the stream is the unit of ownership.  Allocated on first use.
   // shared matrices: setup = the batch's one set-up record of the register-tiled forward (+ the outputs of its set-up launch),
@@ -86,39 +84,44 @@ struct Handle {
   struct StreamWs { cudaStream_t s; double *fwd = nullptr, *bwd = nullptr, *aa = nullptr, *park = nullptr, *jvp = nullptr; size_t aa_cap = 0;
                     double *setup = nullptr, *srec = nullptr, *part = nullptr; size_t srec_cap = 0, part_cap = 0; };
   std::vector<StreamWs> sws;
-  int block_bwd = 0, blk_threads = 0; size_t blk_smem = 0;   // KKT-block preconditioned backward (lsqr_precond = 2)
   int *fail_list[RING] = {nullptr}; int fail_cap[RING] = {0};
-  int fast_fwd = 0;  // dense A, polyhedral cones, direct mode: register-tiled forward (fwd_fast.cu)
-  int fast_bwd = 0;  // dense A, polyhedral cones, dense-or-no P: fused single-pass backward (bwd_fast.cu)
-  // forward-mode derivative (bcone_jvp): always the generic kernel (bwd.cu, JVP = true), so structures on the fused backward
-  // need a generic geometry of their own; chosen by the same rule as the generic backward's.  jvp_ok = 0: none fits.
-  int jvp_ok = 0, jvp_threads = 0, jvp_p_in_smem = 0, jvp_vec_global = 0, jvp_ctas = 0, jvp_small = 0, jvp_ctas_small = 0;
-  // values off chip (the tier after every on-chip option): the forward copies each instance's CSR values into its CTA's slab,
-  // the backward / forward-mode LSQR reads them in place from A_vals.  Only 512-thread builds exist for it (no SMALL variant).
-  int fwd_vals_global = 0, bwd_vals_global = 0, jvp_vals_global = 0;
-  size_t jvp_smem = 0, jvp_ws_stride = 0;
   long long launches = 0;
   int last_block_slot = -1;   // ring slot of the last block-preconditioned vjp (its fallback counter is read by bcone_fallback_count)
   unsigned long long *prof = nullptr;   // device [32] phase cycle counters (bcone_set_profile)
   std::string err;
+  bool upload_failed = false;   // set by upload(), read and cleared by upload_status()
 };
 thread_local std::string g_create_err;
 
-template <class T>
-T *upload(Handle *h, const std::vector<T> &v) {
-  if (v.empty()) return nullptr;
-  void *p = nullptr;
-  if (cudaMalloc(&p, v.size() * sizeof(T)) != cudaSuccess) return nullptr;
-  h->allocs.push_back(p);
-  cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
-  return (T *)p;
-}
 int fail(Handle *h, int code, const std::string &msg) {
   if (h) h->err = msg; else g_create_err = msg;
   return code;
 }
 int cuda_fail(Handle *h, cudaError_t e, const char *where) {
   return fail(h, BCONE_ECUDA, std::string(where) + ": " + cudaGetErrorString(e));
+}
+// Device copy of v (nullptr for an empty one).  A failed allocation or copy returns nullptr too and is recorded on the handle:
+// callers upload everything they need and then ask upload_status() once.
+template <class T>
+T *upload(Handle *h, const std::vector<T> &v) {
+  if (v.empty()) return nullptr;
+  void *p = nullptr;
+  cudaError_t e = cudaMalloc(&p, v.size() * sizeof(T));
+  if (e == cudaSuccess) {
+    h->allocs.push_back(p);
+    e = cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
+  }
+  if (e == cudaSuccess) return (T *)p;
+  cudaGetLastError();   // (not left for the next launch check)
+  h->upload_failed = true;
+  h->err = std::string("upload of ") + std::to_string(v.size() * sizeof(T)) + " B failed: " + cudaGetErrorString(e);
+  return nullptr;
+}
+// BCONE_ENOMEM (message in h->err) if an upload since the last call failed
+int upload_status(Handle *h) {
+  const bool failed = h->upload_failed;
+  h->upload_failed = false;
+  return failed ? BCONE_ENOMEM : BCONE_OK;
 }
 Handle::StreamWs *stream_ws(Handle *h, cudaStream_t s) {
   for (auto &w : h->sws) if (w.s == s) return &w;
@@ -151,41 +154,42 @@ extern "C" const char *bcone_last_error(void *handle) {
   return handle ? ((Handle *)handle)->err.c_str() : g_create_err.c_str();
 }
 
-extern "C" int bcone_create(const bcone_desc *d, void **out) {
-  if (!d || !out) return fail(nullptr, BCONE_EINVAL, "null argument");
-  *out = nullptr;
-  if (d->n <= 0 || d->m < 0 || d->nnzA < 0 || !d->A_indptr || (d->nnzA > 0 && !d->A_indices))
-    return fail(nullptr, BCONE_EINVAL, "bad dimensions / missing A structure");
-  if (d->ep < 0 || d->ed < 0) return fail(nullptr, BCONE_EINVAL, "negative cone count");
+namespace {
+// The BCONE_EINVAL checks of bcone_create: nothing is allocated before they pass.  nullptr = valid.
+const char *validate(const bcone_desc *d) {
+  if (d->n <= 0 || d->m < 0 || d->nnzA < 0 || !d->A_indptr || (d->nnzA > 0 && !d->A_indices)) return "bad dimensions / missing A structure";
+  if (d->ep < 0 || d->ed < 0) return "negative cone count";
   const int n = d->n, m = d->m;
-  long long rows = d->z + d->l;
-  int max_psd = 0, psd_total = 0;
+  long long rows = d->z + d->l + 3LL * (d->ep + d->ed);
   for (int i = 0; i < d->nq; i++) rows += d->q[i];
-  for (int i = 0; i < d->ns; i++) { int k = d->s[i]; rows += (long long)k * (k + 1) / 2; max_psd = std::max(max_psd, k); psd_total += k * k + k; }
-  const int exp_start = (int)rows;
-  rows += 3LL * (d->ep + d->ed);
-  if (rows != m) return fail(nullptr, BCONE_EINVAL, "cone dimensions do not add up to m");
-  if (d->A_indptr[0] != 0 || d->A_indptr[m] != d->nnzA) return fail(nullptr, BCONE_EINVAL, "A_indptr inconsistent with nnzA");
-  if (cudaSetDevice(d->device) != cudaSuccess) return fail(nullptr, BCONE_ECUDA, "cudaSetDevice failed (no CUDA device?)");
-  cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, d->device) != cudaSuccess) return fail(nullptr, BCONE_ECUDA, "cudaGetDeviceProperties failed");
+  for (int i = 0; i < d->ns; i++) rows += (long long)d->s[i] * (d->s[i] + 1) / 2;
+  if (rows != m) return "cone dimensions do not add up to m";
+  if (d->A_indptr[0] != 0 || d->A_indptr[m] != d->nnzA) return "A_indptr inconsistent with nnzA";
+  for (int i = 0; i < m; i++) {
+    if (d->A_indptr[i + 1] < d->A_indptr[i] || d->A_indptr[i + 1] > d->nnzA) return "A_indptr not monotone";   // (it ends at nnzA)
+    for (int k = d->A_indptr[i]; k < d->A_indptr[i + 1]; k++)
+      if (d->A_indices[k] < 0 || d->A_indices[k] >= n) return "A column index out of range";
+  }
+  if (d->P_indptr && d->nnzP > 0)
+    for (int i = 0; i < n; i++) for (int k = d->P_indptr[i]; k < d->P_indptr[i + 1]; k++)
+      if (d->P_indices[k] < i || d->P_indices[k] >= n) return "P must be upper triangular CSR";
+  return nullptr;
+}
 
-  Handle *h = new Handle();
-  h->device = d->device; h->max_batch = d->max_batch; h->num_sms = prop.multiProcessorCount;
-  h->psd_total = psd_total;
+// Host-side structure analysis (CSR -> CSC views, dense-pattern detection, cone block table) and its upload into h->S.
+// The caller checks upload_status() afterwards.
+void analyse_and_upload(Handle *h, const bcone_desc *d) {
+  const int n = d->n, m = d->m;
   DevStruct &S = h->S;
   S.n = n; S.m = m; S.nnzA = d->nnzA; S.nnzP = d->P_indptr ? d->nnzP : 0;
-  S.z = d->z; S.l = d->l; S.nq = d->nq; S.ns = d->ns; S.max_psd = max_psd;
-  S.ep = d->ep; S.ed = d->ed; S.exp_start = exp_start;
-  // --- host-side structure analysis ---
+  S.z = d->z; S.l = d->l; S.nq = d->nq; S.ns = d->ns;
+  S.ep = d->ep; S.ed = d->ed;
   std::vector<int> indptr(d->A_indptr, d->A_indptr + m + 1), indices(d->A_indices, d->A_indices + d->nnzA);
   std::vector<int> rowof(d->nnzA), colptr(n + 1, 0), rowidx(d->nnzA), perm(d->nnzA);
   bool dense = (long long)d->nnzA == (long long)m * n && d->nnzA > 0;
   for (int i = 0; i < m; i++) {
-    if (indptr[i + 1] < indptr[i]) { delete h; return fail(nullptr, BCONE_EINVAL, "A_indptr not monotone"); }
     for (int k = indptr[i]; k < indptr[i + 1]; k++) {
       int j = indices[k];
-      if (j < 0 || j >= n) { delete h; return fail(nullptr, BCONE_EINVAL, "A column index out of range"); }
       rowof[k] = i; colptr[j + 1]++;
       if (dense && j != k - indptr[i]) dense = false;
     }
@@ -198,21 +202,21 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
   }
   S.dense = dense ? 1 : 0;
   std::vector<int> ctype, cstart, csize, corder;
-  {
-    int off = d->z + d->l;
-    for (int i = 0; i < d->nq; i++) { ctype.push_back(BC_CSOC); cstart.push_back(off); csize.push_back(d->q[i]); corder.push_back(0); off += d->q[i]; }
-    for (int i = 0; i < d->ns; i++) { int k = d->s[i], sz = k * (k + 1) / 2; ctype.push_back(BC_CPSD); cstart.push_back(off); csize.push_back(sz); corder.push_back(k); off += sz; }
+  int off = d->z + d->l;
+  for (int i = 0; i < d->nq; i++) { ctype.push_back(BC_CSOC); cstart.push_back(off); csize.push_back(d->q[i]); corder.push_back(0); off += d->q[i]; }
+  for (int i = 0; i < d->ns; i++) {
+    int k = d->s[i], sz = k * (k + 1) / 2;
+    ctype.push_back(BC_CPSD); cstart.push_back(off); csize.push_back(sz); corder.push_back(k); off += sz;
+    S.max_psd = std::max(S.max_psd, k); h->psd_total += k * k + k;
   }
+  S.exp_start = off;
   S.ncones = (int)ctype.size();
   S.A_indptr = upload(h, indptr); S.A_indices = upload(h, indices); S.A_rowof = upload(h, rowof);
   S.At_colptr = upload(h, colptr); S.At_rowidx = upload(h, rowidx); S.At_perm = upload(h, perm);
   S.cone_type = upload(h, ctype); S.cone_start = upload(h, cstart); S.cone_size = upload(h, csize); S.cone_order = upload(h, corder);
   if (S.nnzP > 0) {
     std::vector<int> pptr(d->P_indptr, d->P_indptr + n + 1), pidx(d->P_indices, d->P_indices + S.nnzP), prow(S.nnzP);
-    for (int i = 0; i < n; i++) for (int k = pptr[i]; k < pptr[i + 1]; k++) {
-      if (pidx[k] < i || pidx[k] >= n) { bcone_destroy(h); return fail(nullptr, BCONE_EINVAL, "P must be upper triangular CSR"); }
-      prow[k] = i;
-    }
+    for (int i = 0; i < n; i++) for (int k = pptr[i]; k < pptr[i + 1]; k++) prow[k] = i;
     S.P_indptr = upload(h, pptr); S.P_indices = upload(h, pidx); S.P_rowof = upload(h, prow);
     // CSC view of the upper triangle + dense-pattern detection (row-major full upper triangle)
     std::vector<int> pc(n + 1, 0), pr(S.nnzP), pp(S.nnzP);
@@ -226,139 +230,175 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
     S.Pt_colptr = upload(h, pc); S.Pt_rowidx = upload(h, pr); S.Pt_perm = upload(h, pp);
     S.p_dense = pd ? 1 : 0;
   }
-  if (cudaMalloc((void **)&h->counters, Handle::RING * 4 * sizeof(int)) != cudaSuccess) { bcone_destroy(h); return fail(nullptr, BCONE_ENOMEM, "cudaMalloc counters"); }
-  h->allocs.push_back(h->counters);
+}
 
-  // --- launch geometry: threads by problem size, shared memory must hold the whole instance ---
-  const size_t smem_cap = prop.sharedMemPerBlockOptin;
-  int threads = d->nnzA >= 8192 ? 512 : (d->nnzA >= 1024 ? 256 : 128);
-  while (threads < 512 && threads < n) threads *= 2;  // transposed products want one lane per column
-  const int npoly = d->z + d->l;
+// What the tier searches start from, besides the structure in h->S.
+struct Limits {
+  size_t smem_cap;   // opt-in shared memory per block: must hold what a tier keeps on chip
+  int threads;       // by problem size; the searches halve it down to 64
+  // Last tier, for instances whose CSR values do not fit next to the rest: the values in global memory (L2 when the grid's
+  // working set fits, HBM otherwise), the same rule for everything else.  Tried only after every on-chip option has failed;
+  // BCONE_VALUES_GLOBAL=1 selects it for every generic kernel of a structure that would fit on chip (a test hook).
+  int vals_lo;
+};
+Limits limits(const Handle *h, size_t smem_cap) {
+  const DevStruct &S = h->S;
+  int threads = S.nnzA >= 8192 ? 512 : (S.nnzA >= 1024 ? 256 : 128);
+  while (threads < 512 && threads < S.n) threads *= 2;  // transposed products want one lane per column
+  const char *vgv = getenv("BCONE_VALUES_GLOBAL");
+  return {smem_cap, threads, (vgv && atoi(vgv)) ? 1 : 0};
+}
+
+// Configures t.big (its fn, threads and smem are set) and, where it applies and keeps more CTAs resident, the 4-CTA/SM build.
+cudaError_t configure_tiers(const Handle *h, TieredPlan &t, const void *small_fn) {
+  const cudaError_t e = configure(t.big);
+  if (e != cudaSuccess) return e;
+  if (h->small_mode != 0 && !t.vals_global && t.big.threads <= 256 && t.big.smem <= 56 * 1024) {
+    t.small = t.big; t.small.fn = small_fn;
+    t.has_small = configure(t.small) == cudaSuccess && t.small.ctas > t.big.ctas;
+  }
+  return cudaSuccess;
+}
+
+// Forward: BCONE_OK, BCONE_EUNSUPPORTED (no tier fits) or BCONE_ECUDA (message set).
+int plan_forward(Handle *h, const Limits &L) {
+  const DevStruct &S = h->S;
+  const int n = S.n, m = S.m, nexp = S.ep + S.ed;
   // DIRECT (everything on chip) if the instance fits; else values on chip with the vectors and the packed Cholesky factor
   // in a per-CTA slab of global memory (two triangular products per iteration read it from L2: n <= 512, i.e. <= 1 MB
   // per CTA); else INDIRECT (conjugate gradients, SCS's "indirect" mode).  BCONE_FWD_MODE=indirect forces the last one.
   const char *fm = getenv("BCONE_FWD_MODE");
   const bool force_indirect = fm && std::string(fm) == "indirect";
-  // Last tier, for instances whose CSR values do not fit next to the rest: the values in global memory (L2 when the grid's
-  // working set fits, HBM otherwise), the same rule for everything else.  Tried only after every on-chip option has failed;
-  // BCONE_VALUES_GLOBAL=1 selects it for every generic kernel of a structure that would fit on chip (a test hook).
-  const char *vgv = getenv("BCONE_VALUES_GLOBAL");
-  const int vals_lo = (vgv && atoi(vgv)) ? 1 : 0;
-  auto pick_fwd = [&]() -> bool {
-    for (int vals = vals_lo; vals <= 1; vals++)
-      for (int ind = 0; ind <= 1; ind++)
-        for (int tt = threads; tt >= 64; tt /= 2) {
-          size_t sm = bc_fwd_smem_bytes(n, m, d->nnzA, tt, max_psd, ind, d->ns, d->ep + d->ed, vals);
-          if (sm <= smem_cap) {
-            h->fwd_threads = tt; h->fwd_smem = sm; h->fwd_indirect = ind; h->fwd_vals_global = vals;
-            // (n <= 512: one thread per column in the transposed triangular product; on the sparse LP with n = 1000 the slab mode
-            //  streams 8 MB of factor per iteration and CTA from HBM and loses to conjugate gradients, while at n = 101 the factor
-            //  stays in L2 and the slab mode wins by a wide margin)
-            if (ind && !force_indirect && n <= 512) { h->fwd_indirect = 0; h->fwd_factor_global = 1; }
-            return true;
-          }
+  TieredPlan &t = h->fwd;
+  for (int vals = L.vals_lo; vals <= 1 && !t.big.threads; vals++)
+    for (int ind = 0; ind <= 1 && !t.big.threads; ind++)
+      for (int tt = L.threads; tt >= 64; tt /= 2) {
+        size_t sm = bc_fwd_smem_bytes(n, m, S.nnzA, tt, S.max_psd, ind, S.ns, nexp, vals);
+        if (sm <= L.smem_cap) {
+          t.big.threads = tt; t.big.smem = sm; t.indirect = ind; t.vals_global = vals;
+          // (n <= 512: one thread per column in the transposed triangular product; on the sparse LP with n = 1000 the slab mode
+          //  streams 8 MB of factor per iteration and CTA from HBM and loses to conjugate gradients, while at n = 101 the factor
+          //  stays in L2 and the slab mode wins by a wide margin)
+          if (ind && !force_indirect && n <= 512) { t.indirect = 0; t.factor_global = 1; }
+          break;
         }
-    return false;
-  };
-  // generic LSQR kernel (bwd.cu): prefer P staged in shared memory, then vectors on chip, then vectors in L2; values off chip last
-  auto pick_generic = [&](int &g_threads, size_t &g_smem, int &g_p_in_smem, int &g_vec_global, int &g_vals_global) -> bool {
-    for (int vals = vals_lo; vals <= 1; vals++)
-      for (int vg = 0; vg <= 1; vg++)
-        for (int psm = (S.nnzP > 0 ? 1 : 0); psm >= 0; psm--)
-          for (int tt = threads; tt >= 64; tt /= 2) {
-            size_t sm = bc_bwd_smem_bytes(n, m, npoly, d->nnzA, psm ? S.nnzP : 0, tt, max_psd, psd_total, d->ep + d->ed, vg, vals);
-            if (sm <= smem_cap) { g_threads = tt; g_smem = sm; g_p_in_smem = psm; g_vec_global = vg; g_vals_global = vals; return true; }
-            if (psm) break;  // do not trade threads for P residency
-          }
-    return false;
-  };
-  auto pick_bwd = [&]() -> bool { return pick_generic(h->bwd_threads, h->bwd_smem, h->p_in_smem, h->bwd_vec_global, h->bwd_vals_global); };
-  // fast backward path: same launch geometry fields, different kernel
-  if (S.dense && S.ncones == 0 && d->ep + d->ed == 0 && n <= 128 && (n % 2) == 0 && (S.nnzP == 0 || S.p_dense)) {
-    for (int tt = threads; tt >= 64; tt /= 2) {
-      size_t sm = bc_bwdf_smem_bytes(n, m, d->nnzA, S.nnzP, tt);
-      if (sm <= smem_cap) { h->fast_bwd = 1; h->bwd_threads = tt; h->bwd_smem = sm; h->p_in_smem = S.nnzP > 0; break; }
-    }
-  }
-  if (h->fast_bwd && S.nnzP > 0 && 6 * (n + m + 1) >= 8 * n + 72) {   // block-preconditioned variant for strongly convex QPs
-    for (int tt = threads; tt >= 128; tt /= 2) {
-      size_t sm = bc_bwdb_smem_bytes(n, m, tt);
-      if (sm <= smem_cap) { h->block_bwd = 1; h->blk_threads = tt; h->blk_smem = sm; break; }
-    }
-  }
-  if (!pick_fwd() || (!h->fast_bwd && !pick_bwd())) {
-    // With values and vectors off chip, what is left in shared memory is the per-CTA scratch: the cone scratch (per-warp PSD
-    // scratch, persistent eigenvectors, exp-cone slots) and the 8 n column partials.  Name the largest PSD order that would fit.
-    auto need = [&](int k, size_t *f, size_t *b) {
-      int pt = 0;
-      for (int i = 0; i < d->ns; i++) { const int kk = std::min(d->s[i], k); pt += kk * kk + kk; }
-      *f = bc_fwd_smem_bytes(n, m, d->nnzA, 64, k, 1, k > 0 ? d->ns : 0, d->ep + d->ed, 1);
-      *b = bc_bwd_smem_bytes(n, m, npoly, d->nnzA, 0, 64, k, pt, d->ep + d->ed, 1, 1);
-      return *f <= smem_cap && *b <= smem_cap;
-    };
-    size_t fb = 0, bb = 0, f2 = 0, b2 = 0;
-    need(max_psd, &fb, &bb);
-    int kfit = -1;
-    for (int k = max_psd; k >= 0 && kfit < 0; k--) if (need(k, &f2, &b2)) kfit = k;
-    char buf[512];
-    if (max_psd > 0 && kfit >= 0)
-      snprintf(buf, sizeof buf, "instance does not fit the engine: even with the CSR values and the vectors in global memory, the on-chip cone scratch "
-               "(per-warp PSD scratch and persistent eigenvectors of PSD order %d) needs fwd %zu B / bwd %zu B, %zu B per CTA available; "
-               "the largest PSD order that fits is %d", max_psd, fb, bb, smem_cap, kfit);
-    else
-      snprintf(buf, sizeof buf, "instance does not fit the engine: even with the CSR values and the vectors in global memory, the on-chip scratch "
-               "(cone scratch and 8 n = %d column partials) needs fwd %zu B / bwd %zu B, %zu B per CTA available", 8 * n, fb, bb, smem_cap);
-    bcone_destroy(h);
-    return fail(nullptr, BCONE_EUNSUPPORTED, buf);
-  }
-  cudaError_t e;
+      }
+  if (!t.big.threads) return BCONE_EUNSUPPORTED;
   // register-tiled forward (fwd_fast.cu) when the structure allows it; BCONE_NO_FAST_FWD=1 keeps the generic kernel
-  if (S.dense && S.ncones == 0 && d->ep + d->ed == 0 && !h->fwd_indirect && !h->fwd_factor_global && bc_fwdf_eligible(n, m) &&
-      bc_fwdf_smem_bytes(n, m) <= smem_cap && !(getenv("BCONE_NO_FAST_FWD") && atoi(getenv("BCONE_NO_FAST_FWD")))) {
-    if (bc_fwdf_configure(n, m, bc_fwdf_smem_bytes(n, m)) == cudaSuccess) {
-      h->fast_fwd = 1; h->fwd_threads = bc_fwdf_threads(); h->fwd_smem = bc_fwdf_smem_bytes(n, m);
+  if (S.dense && S.ncones == 0 && nexp == 0 && !t.indirect && !t.factor_global && bc_fwdf_eligible(n, m) &&
+      bc_fwdf_smem_bytes(n, m) <= L.smem_cap && !(getenv("BCONE_NO_FAST_FWD") && atoi(getenv("BCONE_NO_FAST_FWD")))) {
+    h->fwd_fast = Plan{bc_fwdf_kernel(n, m), bc_fwdf_threads(), bc_fwdf_smem_bytes(n, m)};
+    if (configure(h->fwd_fast) == cudaSuccess) { h->fast_fwd = 1; t = TieredPlan(); return BCONE_OK; }   // (the generic kernel is then never launched)
+  }
+  t.big.fn = bc_fwd_kernel(S.dense, t.indirect, 0, t.vals_global);
+  const cudaError_t e = configure_tiers(h, t, bc_fwd_kernel(S.dense, t.indirect, 1, t.vals_global));
+  if (e != cudaSuccess) return cuda_fail(nullptr, e, "cudaFuncSetAttribute");
+  if (t.indirect || t.factor_global || t.vals_global)
+    t.ws_stride = bc_fwd_ws_doubles(n, m, t.indirect || t.factor_global, t.factor_global, t.vals_global ? S.nnzA : 0);
+  return BCONE_OK;
+}
+
+// Generic LSQR kernel (bwd.cu), as the adjoint or as the forward mode: prefer P staged in shared memory, then vectors on chip,
+// then vectors in L2; values off chip last.  BCONE_OK, BCONE_EUNSUPPORTED (no tier fits) or BCONE_ECUDA (message set).
+int plan_lsqr(Handle *h, const Limits &L, TieredPlan &t, int jvp) {
+  const DevStruct &S = h->S;
+  const int npoly = S.z + S.l;
+  for (int vals = L.vals_lo; vals <= 1 && !t.big.threads; vals++)
+    for (int vg = 0; vg <= 1 && !t.big.threads; vg++)
+      for (int psm = (S.nnzP > 0 ? 1 : 0); psm >= 0 && !t.big.threads; psm--)
+        for (int tt = L.threads; tt >= 64; tt /= 2) {
+          size_t sm = bc_bwd_smem_bytes(S.n, S.m, npoly, S.nnzA, psm ? S.nnzP : 0, tt, S.max_psd, h->psd_total, S.ep + S.ed, vg, vals);
+          if (sm <= L.smem_cap) { t.big.threads = tt; t.big.smem = sm; t.p_in_smem = psm; t.vec_global = vg; t.vals_global = vals; break; }
+          if (psm) break;  // do not trade threads for P residency
+        }
+  if (!t.big.threads) return BCONE_EUNSUPPORTED;
+  t.big.fn = bc_lsqr_kernel(S.dense, 0, jvp, t.vals_global);
+  const cudaError_t e = configure_tiers(h, t, bc_lsqr_kernel(S.dense, 1, jvp, t.vals_global));
+  if (e != cudaSuccess) return cuda_fail(nullptr, e, "cudaFuncSetAttribute");
+  if (t.vec_global) t.ws_stride = bc_bwd_ws_doubles(S.n, S.m, npoly);
+  return BCONE_OK;
+}
+
+// Fused single-pass backward (bwd_fast.cu) and, on top of it, the block-preconditioned variant for strongly convex QPs, where
+// the structure allows them.  Sets fast_bwd / block_bwd; BCONE_ECUDA (message set) if the fused kernel cannot be configured.
+int plan_fast(Handle *h, const Limits &L) {
+  const DevStruct &S = h->S;
+  const int n = S.n, m = S.m;
+  if (!(S.dense && S.ncones == 0 && S.ep + S.ed == 0 && n <= 128 && (n % 2) == 0 && (S.nnzP == 0 || S.p_dense))) return BCONE_OK;
+  for (int tt = L.threads; tt >= 64; tt /= 2) {
+    size_t sm = bc_bwdf_smem_bytes(n, m, S.nnzA, S.nnzP, tt);
+    if (sm <= L.smem_cap) { h->fast_bwd = 1; h->bwd_fast = Plan{bc_bwdf_kernel(n), tt, sm}; break; }
+  }
+  if (!h->fast_bwd) return BCONE_OK;
+  const cudaError_t e = configure(h->bwd_fast);
+  if (e != cudaSuccess) return cuda_fail(nullptr, e, "cudaFuncSetAttribute");
+  if (S.nnzP > 0 && 6 * (n + m + 1) >= 8 * n + 72)
+    for (int tt = L.threads; tt >= 128; tt /= 2) {
+      size_t sm = bc_bwdb_smem_bytes(n, m, tt);
+      if (sm <= L.smem_cap) { h->bwd_block = Plan{bc_bwdb_kernel(), tt, sm}; h->block_bwd = configure(h->bwd_block) == cudaSuccess; break; }
     }
-  }
-  {
-    const char *sc = getenv("BCONE_SMALL_CTA");
-    h->small_mode = sc ? atoi(sc) : 1;
-    const bool allow = h->small_mode != 0;
-    h->fwd_small = allow && !h->fast_fwd && !h->fwd_indirect && !h->fwd_vals_global && h->fwd_threads <= 256 && h->fwd_smem <= 56 * 1024;
-    h->bwd_small = allow && !h->fast_bwd && !h->bwd_vals_global && h->bwd_threads <= 256 && h->bwd_smem <= 56 * 1024;
-  }
-  const int fvg = h->fwd_vals_global, bvg = h->bwd_vals_global;
-  if (h->fwd_small && bc_fwd_configure(S.dense, 0, h->fwd_smem, 1, 0) != cudaSuccess) h->fwd_small = 0;
-  if (h->bwd_small && bc_bwd_configure(S.dense, h->bwd_smem, 1, 0) != cudaSuccess) h->bwd_small = 0;
-  if ((e = bc_fwd_configure(S.dense, h->fwd_indirect, h->fast_fwd ? bc_fwd_smem_bytes(n, m, d->nnzA, 64, max_psd, h->fwd_indirect, d->ns, d->ep + d->ed, fvg) : h->fwd_smem, 0, fvg)) != cudaSuccess ||
-      (e = (h->fast_bwd ? bc_bwdf_configure(n, h->bwd_smem) : bc_bwd_configure(S.dense, h->bwd_smem, 0, bvg))) != cudaSuccess) {
-    std::string msg = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e);
-    bcone_destroy(h);
-    return fail(nullptr, BCONE_ECUDA, msg);
-  }
-  if (h->block_bwd && (e = bc_bwdb_configure(h->blk_smem)) != cudaSuccess) h->block_bwd = 0;
-  if (h->fast_fwd) bc_fwdf_occupancy(n, m, h->fwd_smem, &h->fwd_ctas);
-  else bc_fwd_occupancy(S.dense, h->fwd_indirect, h->fwd_threads, h->fwd_smem, &h->fwd_ctas, 0, fvg);
-  if (h->fast_bwd) bc_bwdf_occupancy(n, h->bwd_threads, h->bwd_smem, &h->bwd_ctas);
-  else bc_bwd_occupancy(S.dense, h->bwd_threads, h->bwd_smem, &h->bwd_ctas, 0, bvg);
-  if (h->fwd_ctas < 1) h->fwd_ctas = 1;
-  if (h->bwd_ctas < 1) h->bwd_ctas = 1;
-  if (h->fwd_small) { bc_fwd_occupancy(S.dense, 0, h->fwd_threads, h->fwd_smem, &h->fwd_ctas_small, 1, 0); if (h->fwd_ctas_small <= h->fwd_ctas) h->fwd_small = 0; }
-  if (h->bwd_small) { bc_bwd_occupancy(S.dense, h->bwd_threads, h->bwd_smem, &h->bwd_ctas_small, 1, 0); if (h->bwd_ctas_small <= h->bwd_ctas) h->bwd_small = 0; }
-  if (h->fwd_indirect || h->fwd_factor_global || fvg)
-    h->fwd_ws_stride = bc_fwd_ws_doubles(n, m, h->fwd_indirect || h->fwd_factor_global, h->fwd_factor_global, fvg ? d->nnzA : 0);
-  if (h->bwd_vec_global && !h->fast_bwd) h->bwd_ws_stride = bc_bwd_ws_doubles(n, m, npoly);
+  return BCONE_OK;
+}
+
+// With values and vectors off chip, what is left in shared memory is the per-CTA scratch: the cone scratch (per-warp PSD
+// scratch, persistent eigenvectors, exp-cone slots) and the 8 n column partials.  Name the largest PSD order that would fit.
+std::string explain_no_fit(const Handle *h, const bcone_desc *d, size_t smem_cap) {
+  const DevStruct &S = h->S;
+  const int n = S.n, m = S.m, max_psd = S.max_psd;
+  auto need = [&](int k, size_t *f, size_t *b) {
+    int pt = 0;
+    for (int i = 0; i < d->ns; i++) { const int kk = std::min(d->s[i], k); pt += kk * kk + kk; }
+    *f = bc_fwd_smem_bytes(n, m, d->nnzA, 64, k, 1, k > 0 ? d->ns : 0, d->ep + d->ed, 1);
+    *b = bc_bwd_smem_bytes(n, m, S.z + S.l, d->nnzA, 0, 64, k, pt, d->ep + d->ed, 1, 1);
+    return *f <= smem_cap && *b <= smem_cap;
+  };
+  size_t fb = 0, bb = 0, f2 = 0, b2 = 0;
+  need(max_psd, &fb, &bb);
+  int kfit = -1;
+  for (int k = max_psd; k >= 0 && kfit < 0; k--) if (need(k, &f2, &b2)) kfit = k;
+  char buf[512];
+  if (max_psd > 0 && kfit >= 0)
+    snprintf(buf, sizeof buf, "instance does not fit the engine: even with the CSR values and the vectors in global memory, the on-chip cone scratch "
+             "(per-warp PSD scratch and persistent eigenvectors of PSD order %d) needs fwd %zu B / bwd %zu B, %zu B per CTA available; "
+             "the largest PSD order that fits is %d", max_psd, fb, bb, smem_cap, kfit);
+  else
+    snprintf(buf, sizeof buf, "instance does not fit the engine: even with the CSR values and the vectors in global memory, the on-chip scratch "
+             "(cone scratch and 8 n = %d column partials) needs fwd %zu B / bwd %zu B, %zu B per CTA available", 8 * n, fb, bb, smem_cap);
+  return buf;
+}
+}  // namespace
+
+extern "C" int bcone_create(const bcone_desc *d, void **out) {
+  if (!d || !out) return fail(nullptr, BCONE_EINVAL, "null argument");
+  *out = nullptr;
+  if (const char *bad = validate(d)) return fail(nullptr, BCONE_EINVAL, bad);
+  if (cudaSetDevice(d->device) != cudaSuccess) return fail(nullptr, BCONE_ECUDA, "cudaSetDevice failed (no CUDA device?)");
+  cudaDeviceProp prop;
+  if (cudaGetDeviceProperties(&prop, d->device) != cudaSuccess) return fail(nullptr, BCONE_ECUDA, "cudaGetDeviceProperties failed");
+
+  Handle *h = new Handle();
+  h->device = d->device; h->max_batch = d->max_batch; h->num_sms = prop.multiProcessorCount;
+  // from here on: an error leaves through this, with the message kept past the handle
+  auto give_up = [&](int code, std::string msg) { bcone_destroy(h); return fail(nullptr, code, msg); };
+  analyse_and_upload(h, d);
+  if (upload_status(h) != BCONE_OK) return give_up(BCONE_ENOMEM, h->err);
+  if (cudaMalloc((void **)&h->counters, Handle::RING * 4 * sizeof(int)) != cudaSuccess) return give_up(BCONE_ENOMEM, "cudaMalloc counters");
+  h->allocs.push_back(h->counters);
+
+  // --- launch geometry: threads by problem size, shared memory must hold the whole instance ---
+  const Limits L = limits(h, prop.sharedMemPerBlockOptin);
+  const char *sc = getenv("BCONE_SMALL_CTA");
+  h->small_mode = sc ? atoi(sc) : 1;
+  const int rfast = plan_fast(h, L);
+  int rc = plan_forward(h, L);
+  const int rb = h->fast_bwd ? rfast : plan_lsqr(h, L, h->bwd, 0);
+  if (rc == BCONE_OK || rb == BCONE_EUNSUPPORTED) rc = rb;   // "does not fit" comes before a CUDA error
+  if (rc == BCONE_EUNSUPPORTED) return give_up(rc, explain_no_fit(h, d, L.smem_cap));
+  if (rc != BCONE_OK) return give_up(rc, g_create_err);
   h->tma_ok = (d->nnzA > 0 && (d->nnzA % 2) == 0 && (size_t)d->nnzA * 8 < (1u << 20)) ? 1 : 0;
   // forward-mode derivative: the generic geometry (the backward's own when the backward is generic).  A structure without
   // one is still accepted; only bcone_jvp refuses it.
-  if (pick_generic(h->jvp_threads, h->jvp_smem, h->jvp_p_in_smem, h->jvp_vec_global, h->jvp_vals_global) &&
-      bc_jvp_configure(S.dense, h->jvp_smem, 0, h->jvp_vals_global) == cudaSuccess) {
-    h->jvp_ok = 1;
-    bc_jvp_occupancy(S.dense, h->jvp_threads, h->jvp_smem, &h->jvp_ctas, 0, h->jvp_vals_global);
-    if (h->jvp_ctas < 1) h->jvp_ctas = 1;
-    h->jvp_small = h->small_mode != 0 && !h->jvp_vals_global && h->jvp_threads <= 256 && h->jvp_smem <= 56 * 1024 && bc_jvp_configure(S.dense, h->jvp_smem, 1, 0) == cudaSuccess;
-    if (h->jvp_small) { bc_jvp_occupancy(S.dense, h->jvp_threads, h->jvp_smem, &h->jvp_ctas_small, 1, 0); if (h->jvp_ctas_small <= h->jvp_ctas) h->jvp_small = 0; }
-    if (h->jvp_vec_global) h->jvp_ws_stride = bc_bwd_ws_doubles(n, m, npoly);
-  }
+  h->jvp_ok = plan_lsqr(h, L, h->jvp, 1) == BCONE_OK;
   cudaGetLastError();   // (a refused configuration is not an error of this call)
   *out = h;
   return BCONE_OK;
@@ -379,9 +419,11 @@ extern "C" int bcone_set_boundary(void *handle, int32_t nnz_aug, const int32_t *
   for (int k = 0; k < h->S.nnzA; k++) if (gather[k] < 0 || gather[k] >= h->S.nnzA) return fail(h, BCONE_EINVAL, "set_boundary: gather out of range");
   for (int r = 0; r < nb; r++) if (b_idx[r] < 0 || b_idx[r] >= h->S.m) return fail(h, BCONE_EINVAL, "set_boundary: b_idx out of range");
   cudaSetDevice(h->device);
-  h->nnz_aug = nnz_aug; h->nb = nb;
+  h->nnz_aug = h->nb = 0;   // (until the maps are in place: ingest then asks for this call again)
   h->d_gather = upload(h, std::vector<int>(gather, gather + h->S.nnzA));
   h->d_bidx = upload(h, std::vector<int>(b_idx, b_idx + nb));
+  if (upload_status(h) != BCONE_OK) return BCONE_ENOMEM;
+  h->nnz_aug = nnz_aug; h->nb = nb;
   return BCONE_OK;
 }
 
@@ -391,8 +433,10 @@ extern "C" int bcone_set_boundary_quad(void *handle, int32_t nnzP_boundary, cons
   if (h->S.nnzP > 0 && (!gatherP || nnzP_boundary < 1)) return fail(h, BCONE_EINVAL, "set_boundary_P: missing gather map");
   for (int k = 0; k < h->S.nnzP; k++) if (gatherP[k] < 0 || gatherP[k] >= nnzP_boundary) return fail(h, BCONE_EINVAL, "set_boundary_P: gather out of range");
   cudaSetDevice(h->device);
-  h->nnzP_b = nnzP_boundary;
+  h->nnzP_b = -1;
   h->d_gatherP = h->S.nnzP > 0 ? upload(h, std::vector<int>(gatherP, gatherP + h->S.nnzP)) : nullptr;
+  if (upload_status(h) != BCONE_OK) return BCONE_ENOMEM;
+  h->nnzP_b = nnzP_boundary;
   return BCONE_OK;
 }
 
@@ -424,6 +468,7 @@ extern "C" int bcone_set_param_maps(void *handle, int32_t P1, const int32_t *A_p
   }
   cudaSetDevice(h->device);
   Handle::PMap *dst[3] = {&h->pmA, &h->pmq, &h->pmP};
+  h->P1 = 0;   // (until all three maps are in place)
   for (int w = 0; w < 3; w++) {
     *dst[w] = Handle::PMap();
     if (!rows[w]) continue;
@@ -432,7 +477,7 @@ extern "C" int bcone_set_param_maps(void *handle, int32_t P1, const int32_t *A_p
     std::vector<double> val(std::max(nz, 1), 0.0);
     for (int e = 0; e < nz; e++) { col[e] = colsv[w][e] | (count[colsv[w][e]] == 1 ? 0x40000000 : 0); val[e] = valsv[w][e]; }   // bit 30: exclusive column
     dst[w]->ptr = upload(h, ptr); dst[w]->col = upload(h, col); dst[w]->val = upload(h, val); dst[w]->rows = rows[w];
-    if (!dst[w]->ptr || !dst[w]->col || !dst[w]->val) return fail(h, BCONE_ENOMEM, "set_param_maps: cudaMalloc");
+    if (upload_status(h) != BCONE_OK) return BCONE_ENOMEM;
   }
   h->P1 = P1;
   return BCONE_OK;
@@ -641,20 +686,17 @@ static int solve_impl(Handle *h, int32_t B, const double *A_vals, const double *
   a.sA = shared ? 0 : h->S.nnzA; a.sP = shared ? 0 : h->S.nnzP;
   int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
   a.counter = ctr; a.use_tma = h->tma_ok && (((uintptr_t)A_vals & 15) == 0);
-  // the 4-CTA/SM build only when the batch does not fit the resident capacity of the 128-register build
-  const int use_small = h->fwd_small && (h->small_mode == 2 || B > h->num_sms * h->fwd_ctas);
-  const int ctas = use_small ? h->fwd_ctas_small : h->fwd_ctas;
-  const int grid = std::min(B, h->num_sms * ctas);
-  const size_t max_grid = (size_t)h->num_sms * std::max(h->fwd_ctas, h->fwd_ctas_small);
+  const Plan &plan = h->fast_fwd ? h->fwd_fast : pick(h->fwd, B, h->num_sms, h->small_mode);
+  const int grid = grid_for(plan, B, h->num_sms);
+  const size_t slabs = h->fast_fwd ? (size_t)h->num_sms * plan.ctas : max_grid(h->fwd, h->num_sms);
   Handle::StreamWs *sw = stream_ws(h, st);
-  a.ws = nullptr; a.ws_stride = (long long)h->fwd_ws_stride; a.prof = h->prof;
-  const int fvg = !h->fast_fwd && h->fwd_vals_global;
-  a.slab_vectors = h->fwd_indirect || h->fwd_factor_global;
-  if (h->fwd_indirect || h->fwd_factor_global || fvg) {
-    if (!ensure_slab(h, &sw->fwd, nullptr, h->fwd_ws_stride * max_grid)) {
+  a.ws = nullptr; a.ws_stride = (long long)h->fwd.ws_stride; a.prof = h->prof;
+  a.slab_vectors = h->fwd.indirect || h->fwd.factor_global;
+  if (h->fwd.indirect || h->fwd.factor_global || h->fwd.vals_global) {
+    if (!ensure_slab(h, &sw->fwd, nullptr, h->fwd.ws_stride * slabs)) {
       char buf[160];
-      snprintf(buf, sizeof buf, "cudaMalloc forward workspace (%zu B: %zu B per CTA x %zu CTAs)", h->fwd_ws_stride * max_grid * sizeof(double),
-               h->fwd_ws_stride * sizeof(double), max_grid);
+      snprintf(buf, sizeof buf, "cudaMalloc forward workspace (%zu B: %zu B per CTA x %zu CTAs)", h->fwd.ws_stride * slabs * sizeof(double),
+               h->fwd.ws_stride * sizeof(double), slabs);
       return fail(h, BCONE_ENOMEM, buf);
     }
     a.ws = sw->fwd;
@@ -663,12 +705,12 @@ static int solve_impl(Handle *h, int32_t B, const double *A_vals, const double *
   if (stg->acceleration_lookback != 0 && stg->max_iters > 1) {
     const int mem = std::abs(stg->acceleration_lookback);
     a.aa_stride = (long long)((aa_ws_doubles(h->S.n + h->S.m + 1, mem) + 1) & ~(size_t)1);
-    if (!ensure_slab(h, &sw->aa, &sw->aa_cap, (size_t)a.aa_stride * max_grid)) return fail(h, BCONE_ENOMEM, "cudaMalloc acceleration workspace");
+    if (!ensure_slab(h, &sw->aa, &sw->aa_cap, (size_t)a.aa_stride * slabs)) return fail(h, BCONE_ENOMEM, "cudaMalloc acceleration workspace");
     a.aa_ws = sw->aa;
   }
   a.park = nullptr;
   if (h->fast_fwd) {   // where the register tile waits while a termination check or an acceleration event runs (128 KB per CTA, L2)
-    if (!ensure_slab(h, &sw->park, nullptr, (size_t)32 * 512 * max_grid)) return fail(h, BCONE_ENOMEM, "cudaMalloc tile parking slab");
+    if (!ensure_slab(h, &sw->park, nullptr, (size_t)32 * 512 * slabs)) return fail(h, BCONE_ENOMEM, "cudaMalloc tile parking slab");
     a.park = sw->park;
   }
   if (shared && h->fast_fwd) {
@@ -686,13 +728,12 @@ static int solve_impl(Handle *h, int32_t B, const double *A_vals, const double *
     int *uctr = h->counters + 4 * (h->slot++ % Handle::RING);
     u.counter = uctr;
     CK(cudaMemsetAsync(uctr, 0, sizeof(int), st), "solve counter (set-up)");
-    CK(bc_fwdf_launch(&u, 1, h->fwd_smem, st), "solve launch (shared set-up)");
+    CK(launch(plan, 1, &u, st), "solve launch (shared set-up)");
     h->launches++;
     a.cache = sw->setup; a.cache_stride = 0; a.cache_reuse = 1;
   }
   CK(cudaMemsetAsync(ctr, 0, sizeof(int), st), "solve counter");
-  if (h->fast_fwd) CK(bc_fwdf_launch(&a, grid, h->fwd_smem, st), "solve launch (fast)");
-  else CK(bc_fwd_launch(&a, h->fwd_indirect, grid, h->fwd_threads, h->fwd_smem, st, use_small, fvg), "solve launch");
+  CK(launch(plan, grid, &a, st), h->fast_fwd ? "solve launch (fast)" : "solve launch");
   h->launches++;
   return BCONE_OK;
 }
@@ -740,11 +781,11 @@ static int vjp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   int *ctr = h->counters + 4 * slot;
   a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
   // (values off chip: nothing of A is staged, use_tma only allows the bulk copy of P)
-  a.use_tma = h->bwd_vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = h->p_in_smem;
+  a.use_tma = h->bwd.vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = h->bwd.p_in_smem;
   CK(cudaSetDevice(h->device), "vjp set device");
-  a.ws = nullptr; a.ws_stride = (long long)h->bwd_ws_stride;
-  if (h->bwd_vec_global && !h->fast_bwd) {
-    if (!ensure_slab(h, &sw->bwd, nullptr, h->bwd_ws_stride * (size_t)h->num_sms * std::max(h->bwd_ctas, h->bwd_ctas_small))) return fail(h, BCONE_ENOMEM, "cudaMalloc backward workspace");
+  a.ws = nullptr; a.ws_stride = (long long)h->bwd.ws_stride;
+  if (h->bwd.vec_global) {
+    if (!ensure_slab(h, &sw->bwd, nullptr, h->bwd.ws_stride * max_grid(h->bwd, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc backward workspace");
     a.ws = sw->bwd;
   }
   a.inst_list = nullptr; a.B_dev = nullptr; a.fail_list = nullptr; a.fail_count = nullptr; a.prof = h->prof;
@@ -758,20 +799,18 @@ static int vjp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
     CK(cudaMemsetAsync(ctr + 1, 0, 3 * sizeof(int), st), "vjp counters");
     h->last_block_slot = slot;
     a.fail_list = h->fail_list[slot]; a.fail_count = ctr + 2;
-    CK(bc_bwdb_launch(&a, std::min(B, h->num_sms), h->blk_threads, h->blk_smem, st), "vjp launch (block)");
+    CK(launch(h->bwd_block, std::min(B, h->num_sms), &a, st), "vjp launch (block)");
     BwdArgs f = a;
     f.st.lsqr_precond = 1; f.counter = ctr + 3; f.inst_list = h->fail_list[slot]; f.B_dev = ctr + 2;
     f.fail_list = nullptr; f.fail_count = nullptr;
-    CK(bc_bwdf_launch(&f, std::min(B, h->num_sms * h->bwd_ctas), h->bwd_threads, h->bwd_smem, st), "vjp launch (fallback)");
+    CK(launch(h->bwd_fast, grid_for(h->bwd_fast, B, h->num_sms), &f, st), "vjp launch (fallback)");
     h->launches += 2;
     return reduce();
   }
   if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // block factorisation not available for this structure
   CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "vjp counter");
-  const int use_small = h->bwd_small && (h->small_mode == 2 || B > h->num_sms * h->bwd_ctas);
-  const int grid = std::min(B, h->num_sms * (use_small ? h->bwd_ctas_small : h->bwd_ctas));
-  if (h->fast_bwd) CK(bc_bwdf_launch(&a, grid, h->bwd_threads, h->bwd_smem, st), "vjp launch (fast)");
-  else CK(bc_bwd_launch(&a, grid, h->bwd_threads, h->bwd_smem, st, use_small, h->bwd_vals_global), "vjp launch");
+  const Plan &plan = h->fast_bwd ? h->bwd_fast : pick(h->bwd, B, h->num_sms, h->small_mode);
+  CK(launch(plan, grid_for(plan, B, h->num_sms), &a, st), h->fast_bwd ? "vjp launch (fast)" : "vjp launch");
   h->launches++;
   return reduce();
 }
@@ -806,19 +845,18 @@ static int jvp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
   a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
   if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // no block-preconditioned forward mode
-  a.use_tma = h->jvp_vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = h->jvp_p_in_smem;
+  a.use_tma = h->jvp.vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = h->jvp.p_in_smem;
   CK(cudaSetDevice(h->device), "jvp set device");
-  a.ws_stride = (long long)h->jvp_ws_stride;
-  if (h->jvp_vec_global) {
+  a.ws_stride = (long long)h->jvp.ws_stride;
+  if (h->jvp.vec_global) {
     Handle::StreamWs *sw = stream_ws(h, st);
-    if (!ensure_slab(h, &sw->jvp, nullptr, h->jvp_ws_stride * (size_t)h->num_sms * std::max(h->jvp_ctas, h->jvp_ctas_small))) return fail(h, BCONE_ENOMEM, "cudaMalloc jvp workspace");
+    if (!ensure_slab(h, &sw->jvp, nullptr, h->jvp.ws_stride * max_grid(h->jvp, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc jvp workspace");
     a.ws = sw->jvp;
   }
   a.prof = h->prof;
   CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "jvp counter");
-  const int use_small = h->jvp_small && (h->small_mode == 2 || B > h->num_sms * h->jvp_ctas);
-  const int grid = std::min(B, h->num_sms * (use_small ? h->jvp_ctas_small : h->jvp_ctas));
-  CK(bc_jvp_launch(&a, grid, h->jvp_threads, h->jvp_smem, st, use_small, h->jvp_vals_global), "jvp launch");
+  const Plan &plan = pick(h->jvp, B, h->num_sms, h->small_mode);
+  CK(launch(plan, grid_for(plan, B, h->num_sms), &a, st), "jvp launch");
   h->launches++;
   return BCONE_OK;
 }
@@ -880,17 +918,18 @@ extern "C" int bcone_path_info(void *handle, int32_t *fwd_path, int32_t *bwd_pat
   if (!h) return BCONE_EINVAL;
   if (fwd_path) {
     if (h->fast_fwd) *fwd_path = 2;
-    else if (h->fwd_vals_global) *fwd_path = h->fwd_indirect ? 6 : (h->fwd_factor_global ? 5 : 4);
-    else *fwd_path = h->fwd_indirect ? 1 : (h->fwd_factor_global ? 3 : 0);
+    else if (h->fwd.vals_global) *fwd_path = h->fwd.indirect ? 6 : (h->fwd.factor_global ? 5 : 4);
+    else *fwd_path = h->fwd.indirect ? 1 : (h->fwd.factor_global ? 3 : 0);
   }
-  if (bwd_path) *bwd_path = h->block_bwd ? 2 : (h->fast_bwd ? 1 : (h->bwd_vals_global ? 3 : 0));
+  if (bwd_path) *bwd_path = h->block_bwd ? 2 : (h->fast_bwd ? 1 : (h->bwd.vals_global ? 3 : 0));
   return BCONE_OK;
 }
 
 extern "C" int bcone_kernel_info(void *handle, int32_t *ft, int32_t *fs, int32_t *fc, int32_t *bt, int32_t *bs, int32_t *bcx) {
   Handle *h = (Handle *)handle;
   if (!h) return BCONE_EINVAL;
-  if (ft) *ft = h->fwd_threads; if (fs) *fs = (int32_t)h->fwd_smem; if (fc) *fc = h->fwd_ctas;
-  if (bt) *bt = h->bwd_threads; if (bs) *bs = (int32_t)h->bwd_smem; if (bcx) *bcx = h->bwd_ctas;
+  const Plan &f = h->fast_fwd ? h->fwd_fast : h->fwd.big, &b = h->fast_bwd ? h->bwd_fast : h->bwd.big;
+  if (ft) *ft = f.threads; if (fs) *fs = (int32_t)f.smem; if (fc) *fc = f.ctas;
+  if (bt) *bt = b.threads; if (bs) *bs = (int32_t)b.smem; if (bcx) *bcx = b.ctas;
   return BCONE_OK;
 }

@@ -586,47 +586,15 @@ extern "C" size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_
   return bwd_smem_doubles(n, m, npoly, nnzA, nnzP_smem, threads, max_psd, psd_total, nexp, vec_global, vals_global) * sizeof(double);
 }
 extern "C" size_t bc_bwd_ws_doubles(int n, int m, int npoly) { return (bwd_vec_doubles(n, m, npoly) + 1) & ~(size_t)1; }
-// vg: the values-off-chip builds (512-thread only)
-#define BWD_DISPATCH(EXPR)                                                     \
-  do {                                                                         \
-    if (vg) { if (dense) { auto k = bwd_kernel<true, false, false, true>; EXPR; } else { auto k = bwd_kernel<false, false, false, true>; EXPR; } } \
-    else if (small_cta) { if (dense) { auto k = bwd_kernel<true, true>; EXPR; } else { auto k = bwd_kernel<false, true>; EXPR; } } \
-    else { if (dense) { auto k = bwd_kernel<true, false>; EXPR; } else { auto k = bwd_kernel<false, false>; EXPR; } }         \
-  } while (0)
-extern "C" cudaError_t bc_bwd_configure(int dense, size_t smem, int small_cta, int vg) {
-  cudaError_t e = cudaSuccess;
-  BWD_DISPATCH(e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  return e;
+// The instantiations that exist: the adjoint and the forward-mode derivative (same kernel, same shared-memory layout, JVP = true)
+// each as the 128-register build, the 4-CTA/SM build and the values-off-chip build (512-thread only).
+template <bool JVP>
+static const void *lsqr_kernel(int dense, int small_cta, int vals_global) {
+  if (small_cta && vals_global) return nullptr;
+  if (vals_global) return dense ? (const void *)bwd_kernel<true, false, JVP, true> : (const void *)bwd_kernel<false, false, JVP, true>;
+  if (small_cta) return dense ? (const void *)bwd_kernel<true, true, JVP> : (const void *)bwd_kernel<false, true, JVP>;
+  return dense ? (const void *)bwd_kernel<true, false, JVP> : (const void *)bwd_kernel<false, false, JVP>;
 }
-extern "C" cudaError_t bc_bwd_occupancy(int dense, int threads, size_t smem, int *ctas_per_sm, int small_cta, int vg) {
-  cudaError_t e = cudaSuccess;
-  BWD_DISPATCH(e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, threads, smem));
-  return e;
-}
-extern "C" cudaError_t bc_bwd_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta, int vg) {
-  const int dense = a->S.dense;
-  BWD_DISPATCH((k<<<grid, threads, smem, stream>>>(*a)));
-  return cudaGetLastError();
-}
-// forward-mode derivative: same kernel, same shared-memory layout, JVP = true
-#define JVP_DISPATCH(EXPR)                                                     \
-  do {                                                                         \
-    if (vg) { if (dense) { auto k = bwd_kernel<true, false, true, true>; EXPR; } else { auto k = bwd_kernel<false, false, true, true>; EXPR; } } \
-    else if (small_cta) { if (dense) { auto k = bwd_kernel<true, true, true>; EXPR; } else { auto k = bwd_kernel<false, true, true>; EXPR; } } \
-    else { if (dense) { auto k = bwd_kernel<true, false, true>; EXPR; } else { auto k = bwd_kernel<false, false, true>; EXPR; } }         \
-  } while (0)
-extern "C" cudaError_t bc_jvp_configure(int dense, size_t smem, int small_cta, int vg) {
-  cudaError_t e = cudaSuccess;
-  JVP_DISPATCH(e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  return e;
-}
-extern "C" cudaError_t bc_jvp_occupancy(int dense, int threads, size_t smem, int *ctas_per_sm, int small_cta, int vg) {
-  cudaError_t e = cudaSuccess;
-  JVP_DISPATCH(e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, threads, smem));
-  return e;
-}
-extern "C" cudaError_t bc_jvp_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta, int vg) {
-  const int dense = a->S.dense;
-  JVP_DISPATCH((k<<<grid, threads, smem, stream>>>(*a)));
-  return cudaGetLastError();
+extern "C" const void *bc_lsqr_kernel(int dense, int small_cta, int jvp, int vals_global) {
+  return jvp ? lsqr_kernel<true>(dense, small_cta, vals_global) : lsqr_kernel<false>(dense, small_cta, vals_global);
 }

@@ -354,10 +354,4 @@ __global__ void __launch_bounds__(512, 1) bwd_block_kernel(const __grid_constant
 }
 
 extern "C" size_t bc_bwdb_smem_bytes(int n, int m, int threads) { return bwdb_smem_doubles(n, m, threads) * sizeof(double); }
-extern "C" cudaError_t bc_bwdb_configure(size_t smem) {
-  return cudaFuncSetAttribute(bwd_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-}
-extern "C" cudaError_t bc_bwdb_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream) {
-  bwd_block_kernel<<<grid, threads, smem, stream>>>(*a);
-  return cudaGetLastError();
-}
+extern "C" const void *bc_bwdb_kernel(void) { return (const void *)bwd_block_kernel; }

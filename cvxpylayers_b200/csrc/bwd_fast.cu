@@ -431,16 +431,4 @@ __global__ void __launch_bounds__(512, 1) bwd_fast_kernel(const __grid_constant_
 extern "C" size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads) {
   return bwdf_smem_doubles(n, m, nnzA, nnzP, threads) * sizeof(double);
 }
-extern "C" cudaError_t bc_bwdf_configure(int n, size_t smem) {
-  if (n <= 64) return cudaFuncSetAttribute(bwd_fast_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  return cudaFuncSetAttribute(bwd_fast_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-}
-extern "C" cudaError_t bc_bwdf_occupancy(int n, int threads, size_t smem, int *ctas_per_sm) {
-  if (n <= 64) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, bwd_fast_kernel<1>, threads, smem);
-  return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, bwd_fast_kernel<2>, threads, smem);
-}
-extern "C" cudaError_t bc_bwdf_launch(const BwdArgs *a, int grid, int threads, size_t smem, cudaStream_t stream) {
-  if (a->S.n <= 64) bwd_fast_kernel<1><<<grid, threads, smem, stream>>>(*a);
-  else bwd_fast_kernel<2><<<grid, threads, smem, stream>>>(*a);
-  return cudaGetLastError();
-}
+extern "C" const void *bc_bwdf_kernel(int n) { return n <= 64 ? (const void *)bwd_fast_kernel<1> : (const void *)bwd_fast_kernel<2>; }

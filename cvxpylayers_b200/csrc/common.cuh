@@ -1434,3 +1434,49 @@ __device__ __forceinline__ void project_cones(const DevStruct &S, double *v, dou
     proj_exp_dualblock(v + S.exp_start + 3 * e, e < S.ep, rho + e);
   }
 }
+
+// ----------------------------------------------------------------------------- host entry points
+// Everything api.cu calls in the kernel files, declared once so that the compiler checks each definition against its uses.
+// Per kernel family: the size functions, and one lookup from the variant to the kernel's address (nullptr: no such
+// instantiation).  api.cu configures and launches through that address, so a new kernel variant is registered by adding its
+// row to the family's lookup.
+extern "C" {
+// fwd.cu
+size_t bc_fwd_smem_bytes(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp, int vals_global);
+size_t bc_fwd_ws_doubles(int n, int m, int vectors, int with_factor, int nnzA_global);
+const void *bc_fwd_kernel(int dense, int indirect, int small_cta, int vals_global);
+// fwd_fast.cu
+size_t bc_fwdf_smem_bytes(int n, int m);
+int bc_fwdf_threads(void);
+size_t bc_fwdf_cache_doubles(int n, int m);
+int bc_fwdf_eligible(int n, int m);
+const void *bc_fwdf_kernel(int n, int m);
+// bwd.cu (adjoint and forward mode)
+size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
+                         int vals_global);
+size_t bc_bwd_ws_doubles(int n, int m, int npoly);
+const void *bc_lsqr_kernel(int dense, int small_cta, int jvp, int vals_global);
+// bwd_fast.cu, bwd_block.cu
+size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads);
+const void *bc_bwdf_kernel(int n);
+size_t bc_bwdb_smem_bytes(int n, int m, int threads);
+const void *bc_bwdb_kernel(void);
+// pack.cu
+cudaError_t bc_b2e(const double *in, double *out, int K, int B, int ldo, int roff, const int *smap, const int *dmap, double sign, long long ldb,
+                   cudaStream_t st);
+cudaError_t bc_e2b(const double *in, double *out, int K, int B, int ldi, int roff, const int *smap, const int *dmap, double sign, long long ldb,
+                   cudaStream_t st);
+cudaError_t bc_p2e(const double *p, const int *rptr, const int *cols, const double *vals, double *out, int K, int B, int ldo, int roff,
+                   const int *smap, const int *dmap, double sign, long long ldp, cudaStream_t st);
+cudaError_t bc_e2p(const double *in, const int *rptr, const int *cols, const double *vals, double *dp, int K, int B, int ldi, int roff,
+                   const int *smap, const int *dmap, double sign, int skip, long long ldp, cudaStream_t st);
+cudaError_t bc_rows_from_param(const double *param, long long stride, const int *map, int K, int B, int op, double *rows, cudaStream_t st);
+cudaError_t bc_param_from_rows(const double *grows, const double *param, long long stride, const int *map, int K, int B, int op, double *gparam,
+                               cudaStream_t st);
+cudaError_t bc_gather_cols(const double *in, long long ld, const int *map, const double *scale, int K, int B, int op, double *out, cudaStream_t st);
+cudaError_t bc_scatter_cols(const double *gout, const double *out, long long ld, const int *map, const double *scale, int K, int B, int op, double *gin,
+                            cudaStream_t st);
+// shared.cu
+size_t bc_shared_part_doubles(const DevStruct *S, int B);
+cudaError_t bc_shared_grad(const DevStruct *S, const double *rec, const double *x, int B, double *dA, double *dP, double *part, cudaStream_t st);
+}

@@ -666,7 +666,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) fwd_kernel(c
   }
 }
 
-// ----------------------------------------------------------------------------- host launcher
+// ----------------------------------------------------------------------------- host entry points
 extern "C" size_t bc_fwd_smem_bytes(int n, int m, int nnzA, int threads, int max_psd, int indirect, int ns, int nexp, int vals_global) {
   return fwd_smem_doubles(n, m, nnzA, threads, max_psd, indirect, ns, nexp, vals_global) * sizeof(double);
 }
@@ -676,37 +676,15 @@ extern "C" size_t bc_fwd_ws_doubles(int n, int m, int vectors, int with_factor, 
          (with_factor ? (((size_t)n * (n + 1) / 2 + 1) & ~(size_t)1) : 0);
 }
 
-// vg: the values-off-chip builds (512-thread only: the tier serves large instances)
-#define FWD_DISPATCH(EXPR)                                        \
-  do {                                                            \
-    if (vg) {                                                     \
-      if (dense && indirect) { auto k = fwd_kernel<true, true, false, true>; EXPR; }    \
-      else if (dense) { auto k = fwd_kernel<true, false, false, true>; EXPR; }        \
-      else if (indirect) { auto k = fwd_kernel<false, true, false, true>; EXPR; }     \
-      else { auto k = fwd_kernel<false, false, false, true>; EXPR; }                  \
-    }                                                             \
-    else if (small_cta && !indirect) {                            \
-      if (dense) { auto k = fwd_kernel<true, false, true>; EXPR; }             \
-      else { auto k = fwd_kernel<false, false, true>; EXPR; }                  \
-    }                                                             \
-    else if (dense && indirect) { auto k = fwd_kernel<true, true>; EXPR; }   \
-    else if (dense) { auto k = fwd_kernel<true, false>; EXPR; }              \
-    else if (indirect) { auto k = fwd_kernel<false, true>; EXPR; }           \
-    else { auto k = fwd_kernel<false, false>; EXPR; }                        \
-  } while (0)
-
-extern "C" cudaError_t bc_fwd_configure(int dense, int indirect, size_t smem, int small_cta, int vg) {
-  cudaError_t e = cudaSuccess;
-  FWD_DISPATCH(e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  return e;
-}
-extern "C" cudaError_t bc_fwd_occupancy(int dense, int indirect, int threads, size_t smem, int *ctas_per_sm, int small_cta, int vg) {
-  cudaError_t e = cudaSuccess;
-  FWD_DISPATCH(e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, threads, smem));
-  return e;
-}
-extern "C" cudaError_t bc_fwd_launch(const FwdArgs *a, int indirect, int grid, int threads, size_t smem, cudaStream_t stream, int small_cta, int vg) {
-  const int dense = a->S.dense;
-  FWD_DISPATCH((k<<<grid, threads, smem, stream>>>(*a)));
-  return cudaGetLastError();
+// The instantiations that exist.  small_cta: the 4-CTA/SM build, direct solve with the values on chip only; vals_global: the
+// values-off-chip builds (512-thread only: the tier serves large instances).
+extern "C" const void *bc_fwd_kernel(int dense, int indirect, int small_cta, int vals_global) {
+  if (small_cta && (indirect || vals_global)) return nullptr;
+  if (vals_global) {
+    if (dense) return indirect ? (const void *)fwd_kernel<true, true, false, true> : (const void *)fwd_kernel<true, false, false, true>;
+    return indirect ? (const void *)fwd_kernel<false, true, false, true> : (const void *)fwd_kernel<false, false, false, true>;
+  }
+  if (small_cta) return dense ? (const void *)fwd_kernel<true, false, true> : (const void *)fwd_kernel<false, false, true>;
+  if (dense) return indirect ? (const void *)fwd_kernel<true, true> : (const void *)fwd_kernel<true, false>;
+  return indirect ? (const void *)fwd_kernel<false, true> : (const void *)fwd_kernel<false, false>;
 }

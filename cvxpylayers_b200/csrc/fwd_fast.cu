@@ -1009,14 +1009,12 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
   }
 }
 
-// ----------------------------------------------------------------------------- host launcher
+// ----------------------------------------------------------------------------- host entry points
 // Specialised geometries (compile-time offsets); anything else runs the <0, 0> instantiation.
-#define FWDF_DISPATCH(n, m, EXPR)                                                      \
-  do {                                                                                 \
-    const Geo<0, 0> g0(n, m);                                                          \
-    if (g0.CT() == 10 && g0.RTu() == 50) { auto k = fwd_fast_kernel<10, 50>; EXPR; }   \
-    else { auto k = fwd_fast_kernel<0, 0>; EXPR; }                                     \
-  } while (0)
+extern "C" const void *bc_fwdf_kernel(int n, int m) {
+  const Geo<0, 0> g0(n, m);
+  return g0.CT() == 10 && g0.RTu() == 50 ? (const void *)fwd_fast_kernel<10, 50> : (const void *)fwd_fast_kernel<0, 0>;
+}
 
 // (sizes come from the geometry type the launch will instantiate: the padded Kinv stride exists only in the compile-time one)
 #define FWDF_GEO(n, m, EXPR)                                                                 \
@@ -1039,18 +1037,4 @@ extern "C" size_t bc_fwdf_cache_doubles(int n, int m) { size_t r = 0; FWDF_GEO(n
 extern "C" int bc_fwdf_eligible(int n, int m) {
   const Geo<0, 0> g(n, m);
   return g.ok(n, m) && g.CT() * g.RTu() >= FT / 2;
-}
-extern "C" cudaError_t bc_fwdf_configure(int n, int m, size_t smem) {
-  cudaError_t e = cudaSuccess;
-  FWDF_DISPATCH(n, m, e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  return e;
-}
-extern "C" cudaError_t bc_fwdf_occupancy(int n, int m, size_t smem, int *ctas_per_sm) {
-  cudaError_t e = cudaSuccess;
-  FWDF_DISPATCH(n, m, e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, FT, smem));
-  return e;
-}
-extern "C" cudaError_t bc_fwdf_launch(const FwdArgs *a, int grid, size_t smem, cudaStream_t stream) {
-  FWDF_DISPATCH(a->S.n, a->S.m, (k<<<grid, FT, smem, stream>>>(*a)));
-  return cudaGetLastError();
 }

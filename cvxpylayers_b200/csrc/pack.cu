@@ -7,7 +7,7 @@
 // kernels are that re-packing, fused with the sign flip (A = -A_cvx), the CSC->CSR gather and
 // the b_idx scatter: HBM-bound tiled transposes, 128-bit loads along the batch axis.
 #include <cuda_runtime.h>
-#include <stdint.h>
+#include "common.cuh"
 
 #define TK 32  // rows of the boundary matrix per tile
 #define TI 64  // batch entries per tile
