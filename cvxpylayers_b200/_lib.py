@@ -19,7 +19,7 @@ _f64p = C.POINTER(C.c_double)
 EXPORTS = [
     "bcone_default_settings", "bcone_create", "bcone_destroy", "bcone_last_error", "bcone_set_boundary", "bcone_set_boundary_quad",
     "bcone_ingest", "bcone_emit", "bcone_ingest_pitched", "bcone_emit_pitched", "bcone_peer_alloc", "bcone_peer_open", "bcone_peer_close",
-    "bcone_peer_free", "bcone_copy2d_async", "bcone_rows_from_param", "bcone_param_from_rows", "bcone_gather_cols", "bcone_scatter_cols", "bcone_set_param_maps", "bcone_ingest_params", "bcone_emit_params", "bcone_solve", "bcone_solve_warm", "bcone_solve_cached", "bcone_cache_bytes", "bcone_vjp", "bcone_jvp", "bcone_launch_count", "bcone_fallback_count", "bcone_kernel_info", "bcone_path_info", "bcone_memcpy2d", "bcone_set_profile",
+    "bcone_peer_free", "bcone_copy2d_async", "bcone_rows_from_param", "bcone_param_from_rows", "bcone_gather_cols", "bcone_scatter_cols", "bcone_set_param_maps", "bcone_ingest_params", "bcone_emit_params", "bcone_solve", "bcone_solve_warm", "bcone_solve_cached", "bcone_cache_bytes", "bcone_vjp", "bcone_jvp", "bcone_launch_count", "bcone_fallback_count", "bcone_kernel_info", "bcone_path_info", "bcone_small_cta_info", "bcone_memcpy2d", "bcone_set_profile",
     "bcone_solve_shared", "bcone_vjp_shared", "bcone_jvp_shared", "bcone_ingest_params_shared", "bcone_emit_params_shared",
 ]
 
@@ -140,6 +140,8 @@ def load() -> C.CDLL:
     lib.bcone_kernel_info.restype = C.c_int
     lib.bcone_path_info.argtypes = [vp, _i32p, _i32p]
     lib.bcone_path_info.restype = C.c_int
+    lib.bcone_small_cta_info.argtypes = [vp, _i32p, _i32p]
+    lib.bcone_small_cta_info.restype = C.c_int
     _lib = lib
     return lib
 

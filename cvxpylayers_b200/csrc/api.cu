@@ -925,6 +925,14 @@ extern "C" int bcone_path_info(void *handle, int32_t *fwd_path, int32_t *bwd_pat
   return BCONE_OK;
 }
 
+extern "C" int bcone_small_cta_info(void *handle, int32_t *fwd_small_ctas, int32_t *bwd_small_ctas) {
+  Handle *h = (Handle *)handle;
+  if (!h) return BCONE_EINVAL;
+  if (fwd_small_ctas) *fwd_small_ctas = h->fwd.has_small ? h->fwd.small.ctas : 0;
+  if (bwd_small_ctas) *bwd_small_ctas = h->bwd.has_small ? h->bwd.small.ctas : 0;
+  return BCONE_OK;
+}
+
 extern "C" int bcone_kernel_info(void *handle, int32_t *ft, int32_t *fs, int32_t *fc, int32_t *bt, int32_t *bs, int32_t *bcx) {
   Handle *h = (Handle *)handle;
   if (!h) return BCONE_EINVAL;

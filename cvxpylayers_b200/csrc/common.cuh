@@ -1259,9 +1259,9 @@ __device__ inline double exp_calc_grad(const double *v, double *x, double rho) {
   return x[0] + x[1] * log(x[1] / x[2]);
 }
 __device__ inline double exp_h(double r, double s, double t, double rho, double *y, double *mu) {
-  const double E = exp(rho);
-  *y = (r + t * E) / (rho + E * E);
-  *mu = *y * E - t;
+  const double E = exp(rho), id = 1.0 / (rho + E * E);
+  *y = (r + t * E) * id;
+  *mu = (r * E - t * rho) * id;   // = y e^rho - t without its cancellation once y e^rho ~ t
   return *y + *mu * E * (1.0 - rho) - s;
 }
 // Newton on h(rho) = 0 (rho = x / y of the projection p = (rho y, y, y e^rho); h is the stationarity residual of the
@@ -1305,9 +1305,11 @@ __device__ inline bool exp_newton_rho(double r, double s, double t, double *rho0
   const double E = exp(rho);
   const double px = y * rho, py = y, pz = y * E;
   const double dx = r - px, dy = s - py, dz = t - pz;           // must be mu (E, (1 - rho) E, -1), mu >= 0
-  const double mu2 = -dz;
+  // the normal divided by max(1, e^rho): mu2 = -dz would carry the rounding of t - y e^rho, times e^rho, into dx
+  const double na = E >= 1.0 ? 1.0 : E, n0 = na, n1 = na * (1.0 - rho), n2 = E >= 1.0 ? -1.0 / E : -1.0;
+  const double nn = sqrt(n0 * n0 + n1 * n1 + n2 * n2), mu2 = (dx * n0 + dy * n1 + dz * n2) / nn;
   if (!(mu2 >= -1e-13 * scale)) return false;
-  if (fabs(dx - mu2 * E) > 1e-9 * scale || fabs(dy - mu2 * E * (1.0 - rho)) > 1e-9 * scale) return false;
+  if (fabs(dx - mu2 * n0 / nn) > 1e-9 * scale || fabs(dy - mu2 * n1 / nn) > 1e-9 * scale || fabs(dz - mu2 * n2 / nn) > 1e-9 * scale) return false;
   if (fabs(px * dx + py * dy + pz * dz) > 1e-9 * scale * scale) return false;
   x[0] = px; x[1] = py; x[2] = pz;
   if (rho0) *rho0 = rho;
@@ -1327,7 +1329,7 @@ __device__ inline bool exp_newton_multi(double r, double s, double t, double *rh
 }
 // v <- Pi_{K_exp}(v); returns the case (0 inside, 1 polar, 2 analytic face, 3 iterative).  rho0: optional warm start
 // slot of this cone (NaN = none), updated when the Newton path was taken.
-__device__ inline int proj_exp(double *v, double *rho0 = nullptr) {
+__device__ inline int proj_exp_unit(double *v, double *rho0) {
   const double r = v[0], s = v[1], t = v[2];
   if ((s > 0 && s * exp(fmin(r / s, 700.0)) - t <= 1e-13) || (r <= 0 && s == 0 && t >= 0)) return 0;
   if ((r > 0 && r * exp(fmin(s / r, 700.0)) + 2.718281828459045 * t <= 1e-13) || (r == 0 && s <= 0 && t <= 0)) { v[0] = v[1] = v[2] = 0; return 1; }
@@ -1359,10 +1361,32 @@ __device__ inline int proj_exp(double *v, double *rho0 = nullptr) {
   v[0] = x[0]; v[1] = x[1]; v[2] = x[2];
   return 3;
 }
+// The projection is positively homogeneous and its Jacobian homogeneous of degree 0: both work on v / 2^k with max|v_i| in
+// [1, 2), so that the absolute thresholds of proj_exp_unit (the 1e-13 case tests, the 1e-12 face test, the Newton and
+// bisection tolerances) are relative to |v|; a power of two keeps the scaling exact.
+// 2^-k and 2^k are built from the exponent field (k clamped so both stay normal); returns 2^k.
+__device__ inline double exp_unit_scale(const double *v, double *u) {
+  const double m = fmax(fabs(v[0]), fmax(fabs(v[1]), fabs(v[2])));
+  const int k = m > 0.0 ? min(max((int)((__double_as_longlong(m) >> 52) & 0x7ff) - 1023, -1000), 1000) : 0;
+  const double down = __longlong_as_double((long long)(1023 - k) << 52);
+#pragma unroll
+  for (int i = 0; i < 3; i++) u[i] = v[i] * down;
+  return __longlong_as_double((long long)(1023 + k) << 52);
+}
+__device__ inline int proj_exp(double *v, double *rho0 = nullptr) {
+  double u[3];
+  const double up = exp_unit_scale(v, u);
+  const int cs = proj_exp_unit(u, rho0);
+#pragma unroll
+  for (int i = 0; i < 3; i++) v[i] = u[i] * up;
+  return cs;
+}
 // J (3x3 row-major) = D Pi_{K_exp}(v)
-__device__ inline void dproj_exp_mat(const double *v, double *J) {
+__device__ inline void dproj_exp_mat(const double *v0, double *J) {
+  double v[3];
+  exp_unit_scale(v0, v);
   double p[3] = {v[0], v[1], v[2]};
-  const int cs = proj_exp(p);
+  const int cs = proj_exp_unit(p, nullptr);
   for (int i = 0; i < 9; i++) J[i] = 0;
   if (cs == 0) { J[0] = J[4] = J[8] = 1.0; return; }
   if (cs == 1) return;

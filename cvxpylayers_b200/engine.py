@@ -140,6 +140,12 @@ class Engine:
     BWD_PATHS = ("bwd_kernel (generic LSQR)", "bwd_fast_kernel (fused single-pass LSQR)", "bwd_block_kernel (KKT-block preconditioned, bwd_fast_kernel fallback)",
                  "bwd_kernel (generic LSQR, values off chip: read in place from A_vals)")
 
+    def small_cta_info(self) -> dict:
+        """CTAs per SM of the 4-CTA/SM builds of the generic forward and adjoint (0: the structure has none)."""
+        f, b = C.c_int32(), C.c_int32()
+        self.lib.bcone_small_cta_info(self.h, C.byref(f), C.byref(b))
+        return {"fwd": f.value, "bwd": b.value}
+
     def path_info(self) -> dict:
         f, b = C.c_int32(), C.c_int32()
         self.lib.bcone_path_info(self.h, C.byref(f), C.byref(b))

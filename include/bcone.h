@@ -254,6 +254,10 @@ int bcone_kernel_info(void *handle, int32_t *fwd_threads, int32_t *fwd_smem, int
  * single-pass LSQR (bwd_fast.cu), 2 KKT-block preconditioned (bwd_block.cu, used when lsqr_precond = 2; falls back to 1 per
  * instance), 3 generic LSQR with the values read in place from A_vals (values off chip; bcone_jvp then runs the same way). */
 int bcone_path_info(void *handle, int32_t *fwd_path, int32_t *bwd_path);
+/* CTAs per SM of the generic forward's and adjoint's 4-CTA/SM build, 0 where the structure has none (more than 256 threads,
+ * more than 56 KB of shared memory, or no gain in resident CTAs).  With BCONE_SMALL_CTA=2 every launch of a kernel that has
+ * that build takes it. */
+int bcone_small_cta_info(void *handle, int32_t *fwd_small_ctas, int32_t *bwd_small_ctas);
 
 #ifdef __cplusplus
 }
