@@ -39,7 +39,7 @@ class BconeSettings(C.Structure):
                 ("max_iters", C.c_int32), ("normalize", C.c_int32), ("adaptive_scale", C.c_int32),
                 ("check_interval", C.c_int32), ("ruiz_passes", C.c_int32), ("lsqr_iter_lim", C.c_int32),
                 ("lsqr_precond", C.c_int32), ("adaptive_check", C.c_int32),
-                ("acceleration_lookback", C.c_int32), ("acceleration_interval", C.c_int32)]
+                ("acceleration_lookback", C.c_int32), ("acceleration_interval", C.c_int32), ("lsmr", C.c_int32)]
 
 
 class EngineUnavailable(RuntimeError):

@@ -76,12 +76,19 @@ struct Handle {
   Plan bwd_fast;    // fast_bwd: dense A, polyhedral cones, dense-or-no P: fused single-pass backward (bwd_fast.cu)
   Plan bwd_block;   // block_bwd: KKT-block preconditioned backward (lsqr_precond = 2)
   int fast_fwd = 0, fast_bwd = 0, block_bwd = 0;
+  // LSMR (settings.lsmr = 1): the same plans for the LSMR kernels, which keep one more N-vector, chosen by the same rules.  A
+  // structure on the fused backward whose fused geometry has no room for that vector runs the generic LSMR kernel
+  // (bwd_lsmr); the block-preconditioned LSMR hands the instances it rejects to whichever of the two runs.
+  TieredPlan bwd_lsmr, jvp_lsmr; int bwd_lsmr_ok = 0, jvp_lsmr_ok = 0;
+  Plan bwd_fast_lsmr, bwd_block_lsmr;
+  int fast_bwd_lsmr = 0, block_bwd_lsmr = 0;
   int small_mode = 1;   // BCONE_SMALL_CTA: 0 disables the 4-CTA/SM builds, 2 forces them
   // Per-stream scratch slabs (one per CTA of the grid): launches on different streams may overlap, launches on one
   // stream cannot, so the stream is the unit of ownership.  Allocated on first use.
   // shared matrices: setup = the batch's one set-up record of the register-tiled forward (+ the outputs of its set-up launch),
   // srec / part = the adjoint's per-instance r, pi_y records and the reduction's partial sums (shared.cu)
   struct StreamWs { cudaStream_t s; double *fwd = nullptr, *bwd = nullptr, *aa = nullptr, *park = nullptr, *jvp = nullptr; size_t aa_cap = 0;
+                    double *bwd_lsmr = nullptr, *jvp_lsmr = nullptr;
                     double *setup = nullptr, *srec = nullptr, *part = nullptr; size_t srec_cap = 0, part_cap = 0; };
   std::vector<StreamWs> sws;
   int *fail_list[RING] = {nullptr}; int fail_cap[RING] = {0};
@@ -148,6 +155,7 @@ extern "C" void bcone_default_settings(bcone_settings *st) {
   st->max_iters = 100000; st->normalize = 1; st->adaptive_scale = 1; st->check_interval = 25;
   st->ruiz_passes = 10; st->lsqr_iter_lim = -1; st->lsqr_precond = 0; st->adaptive_check = 0;
   st->acceleration_lookback = 10; st->acceleration_interval = 10;   // SCS defaults
+  st->lsmr = 0;
 }
 
 extern "C" const char *bcone_last_error(void *handle) {
@@ -298,24 +306,25 @@ int plan_forward(Handle *h, const Limits &L) {
   return BCONE_OK;
 }
 
-// Generic LSQR kernel (bwd.cu), as the adjoint or as the forward mode: prefer P staged in shared memory, then vectors on chip,
-// then vectors in L2; values off chip last.  BCONE_OK, BCONE_EUNSUPPORTED (no tier fits) or BCONE_ECUDA (message set).
-int plan_lsqr(Handle *h, const Limits &L, TieredPlan &t, int jvp) {
+// Generic LSQR kernel (bwd.cu), as the adjoint or as the forward mode, or its LSMR variant (lsmr = 1): prefer P staged in
+// shared memory, then vectors on chip, then vectors in L2; values off chip last.  BCONE_OK, BCONE_EUNSUPPORTED (no tier fits)
+// or BCONE_ECUDA (message set).
+int plan_lsqr(Handle *h, const Limits &L, TieredPlan &t, int jvp, int lsmr) {
   const DevStruct &S = h->S;
   const int npoly = S.z + S.l;
   for (int vals = L.vals_lo; vals <= 1 && !t.big.threads; vals++)
     for (int vg = 0; vg <= 1 && !t.big.threads; vg++)
       for (int psm = (S.nnzP > 0 ? 1 : 0); psm >= 0 && !t.big.threads; psm--)
         for (int tt = L.threads; tt >= 64; tt /= 2) {
-          size_t sm = bc_bwd_smem_bytes(S.n, S.m, npoly, S.nnzA, psm ? S.nnzP : 0, tt, S.max_psd, h->psd_total, S.ep + S.ed, vg, vals);
+          size_t sm = bc_bwd_smem_bytes(S.n, S.m, npoly, S.nnzA, psm ? S.nnzP : 0, tt, S.max_psd, h->psd_total, S.ep + S.ed, vg, vals, lsmr);
           if (sm <= L.smem_cap) { t.big.threads = tt; t.big.smem = sm; t.p_in_smem = psm; t.vec_global = vg; t.vals_global = vals; break; }
           if (psm) break;  // do not trade threads for P residency
         }
   if (!t.big.threads) return BCONE_EUNSUPPORTED;
-  t.big.fn = bc_lsqr_kernel(S.dense, 0, jvp, t.vals_global);
-  const cudaError_t e = configure_tiers(h, t, bc_lsqr_kernel(S.dense, 1, jvp, t.vals_global));
+  t.big.fn = bc_lsqr_kernel(S.dense, 0, jvp, t.vals_global, lsmr);
+  const cudaError_t e = configure_tiers(h, t, bc_lsqr_kernel(S.dense, 1, jvp, t.vals_global, lsmr));
   if (e != cudaSuccess) return cuda_fail(nullptr, e, "cudaFuncSetAttribute");
-  if (t.vec_global) t.ws_stride = bc_bwd_ws_doubles(S.n, S.m, npoly);
+  if (t.vec_global) t.ws_stride = bc_bwd_ws_doubles(S.n, S.m, npoly, lsmr);
   return BCONE_OK;
 }
 
@@ -326,8 +335,8 @@ int plan_fast(Handle *h, const Limits &L) {
   const int n = S.n, m = S.m;
   if (!(S.dense && S.ncones == 0 && S.ep + S.ed == 0 && n <= 128 && (n % 2) == 0 && (S.nnzP == 0 || S.p_dense))) return BCONE_OK;
   for (int tt = L.threads; tt >= 64; tt /= 2) {
-    size_t sm = bc_bwdf_smem_bytes(n, m, S.nnzA, S.nnzP, tt);
-    if (sm <= L.smem_cap) { h->fast_bwd = 1; h->bwd_fast = Plan{bc_bwdf_kernel(n), tt, sm}; break; }
+    size_t sm = bc_bwdf_smem_bytes(n, m, S.nnzA, S.nnzP, tt, 0);
+    if (sm <= L.smem_cap) { h->fast_bwd = 1; h->bwd_fast = Plan{bc_bwdf_kernel(n, 0), tt, sm}; break; }
   }
   if (!h->fast_bwd) return BCONE_OK;
   const cudaError_t e = configure(h->bwd_fast);
@@ -335,9 +344,27 @@ int plan_fast(Handle *h, const Limits &L) {
   if (S.nnzP > 0 && 6 * (n + m + 1) >= 8 * n + 72)
     for (int tt = L.threads; tt >= 128; tt /= 2) {
       size_t sm = bc_bwdb_smem_bytes(n, m, tt);
-      if (sm <= L.smem_cap) { h->bwd_block = Plan{bc_bwdb_kernel(), tt, sm}; h->block_bwd = configure(h->bwd_block) == cudaSuccess; break; }
+      if (sm <= L.smem_cap) { h->bwd_block = Plan{bc_bwdb_kernel(0), tt, sm}; h->block_bwd = configure(h->bwd_block) == cudaSuccess; break; }
     }
   return BCONE_OK;
+}
+
+// The LSMR variants of the fused and the block-preconditioned backward, where the LSQR ones run.  The fused one keeps one more
+// N-vector, searched for by the same rule; where it does not fit (C2: A and P fill shared memory), the generic LSMR kernel runs
+// the adjoint.  The block-preconditioned one needs no more shared memory than its LSQR twin and takes its geometry; the
+// instances it rejects go to the fused LSMR kernel, or to the generic one (bcone_create checks that one of them exists).
+void plan_fast_lsmr(Handle *h, const Limits &L) {
+  const DevStruct &S = h->S;
+  const int n = S.n, m = S.m;
+  if (!h->fast_bwd) return;
+  for (int tt = L.threads; tt >= 64; tt /= 2) {
+    const size_t sm = bc_bwdf_smem_bytes(n, m, S.nnzA, S.nnzP, tt, 1);
+    if (sm <= L.smem_cap) { h->bwd_fast_lsmr = Plan{bc_bwdf_kernel(n, 1), tt, sm}; h->fast_bwd_lsmr = configure(h->bwd_fast_lsmr) == cudaSuccess; break; }
+  }
+  if (h->block_bwd) {
+    h->bwd_block_lsmr = h->bwd_block; h->bwd_block_lsmr.fn = bc_bwdb_kernel(1);
+    h->block_bwd_lsmr = configure(h->bwd_block_lsmr) == cudaSuccess;
+  }
 }
 
 // With values and vectors off chip, what is left in shared memory is the per-CTA scratch: the cone scratch (per-warp PSD
@@ -349,7 +376,7 @@ std::string explain_no_fit(const Handle *h, const bcone_desc *d, size_t smem_cap
     int pt = 0;
     for (int i = 0; i < d->ns; i++) { const int kk = std::min(d->s[i], k); pt += kk * kk + kk; }
     *f = bc_fwd_smem_bytes(n, m, d->nnzA, 64, k, 1, k > 0 ? d->ns : 0, d->ep + d->ed, 1);
-    *b = bc_bwd_smem_bytes(n, m, S.z + S.l, d->nnzA, 0, 64, k, pt, d->ep + d->ed, 1, 1);
+    *b = bc_bwd_smem_bytes(n, m, S.z + S.l, d->nnzA, 0, 64, k, pt, d->ep + d->ed, 1, 1, 0);
     return *f <= smem_cap && *b <= smem_cap;
   };
   size_t fb = 0, bb = 0, f2 = 0, b2 = 0;
@@ -391,14 +418,19 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
   h->small_mode = sc ? atoi(sc) : 1;
   const int rfast = plan_fast(h, L);
   int rc = plan_forward(h, L);
-  const int rb = h->fast_bwd ? rfast : plan_lsqr(h, L, h->bwd, 0);
+  const int rb = h->fast_bwd ? rfast : plan_lsqr(h, L, h->bwd, 0, 0);
   if (rc == BCONE_OK || rb == BCONE_EUNSUPPORTED) rc = rb;   // "does not fit" comes before a CUDA error
   if (rc == BCONE_EUNSUPPORTED) return give_up(rc, explain_no_fit(h, d, L.smem_cap));
   if (rc != BCONE_OK) return give_up(rc, g_create_err);
   h->tma_ok = (d->nnzA > 0 && (d->nnzA % 2) == 0 && (size_t)d->nnzA * 8 < (1u << 20)) ? 1 : 0;
   // forward-mode derivative: the generic geometry (the backward's own when the backward is generic).  A structure without
   // one is still accepted; only bcone_jvp refuses it.
-  h->jvp_ok = plan_lsqr(h, L, h->jvp, 1) == BCONE_OK;
+  h->jvp_ok = plan_lsqr(h, L, h->jvp, 1, 0) == BCONE_OK;
+  // LSMR (settings.lsmr = 1): likewise; a structure without an LSMR geometry is accepted, only LSMR calls refuse it
+  plan_fast_lsmr(h, L);
+  h->bwd_lsmr_ok = h->fast_bwd_lsmr || plan_lsqr(h, L, h->bwd_lsmr, 0, 1) == BCONE_OK;
+  if (!h->bwd_lsmr_ok) h->block_bwd_lsmr = 0;   // (no pass for the instances it rejects)
+  h->jvp_lsmr_ok = plan_lsqr(h, L, h->jvp_lsmr, 1, 1) == BCONE_OK;
   cudaGetLastError();   // (a refused configuration is not an error of this call)
   *out = h;
   return BCONE_OK;
@@ -680,7 +712,7 @@ static int solve_impl(Handle *h, int32_t B, const double *A_vals, const double *
   CK(cudaSetDevice(h->device), "solve set device");
   FwdArgs a;
   a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
-  a.x = x; a.y = y; a.s = s; a.status = status; a.iters = iters; a.resid = resid; a.st = *stg;
+  a.x = x; a.y = y; a.s = s; a.status = status; a.iters = iters; a.resid = resid; a.st = kernel_settings(*stg);
   a.x0 = x0; a.y0 = y0; a.s0 = s0;
   a.cache = (double *)cache; a.cache_stride = h->fast_fwd ? (long long)bc_fwdf_cache_doubles(h->S.n, h->S.m) : 0; a.cache_reuse = cache && reuse;
   a.sA = shared ? 0 : h->S.nnzA; a.sP = shared ? 0 : h->S.nnzP;
@@ -756,6 +788,12 @@ static int vjp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !dx || !dy || !dA_vals || !db || !dc || !stg)
     return fail(h, BCONE_EINVAL, "vjp: null argument");
   if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "vjp: structure has P but P_vals is NULL");
+  // the LSQR or the LSMR kernels (settings.lsmr)
+  const bool lsmr = stg->lsmr != 0;
+  if (lsmr && !h->bwd_lsmr_ok) return fail(h, BCONE_EUNSUPPORTED, "vjp: the instance does not fit the LSMR kernels");
+  const TieredPlan &gen = lsmr ? h->bwd_lsmr : h->bwd;
+  const int fast_bwd = lsmr ? h->fast_bwd_lsmr : h->fast_bwd, block_bwd = lsmr ? h->block_bwd_lsmr : h->block_bwd;
+  const Plan &bwd_fast = lsmr ? h->bwd_fast_lsmr : h->bwd_fast, &bwd_block = lsmr ? h->bwd_block_lsmr : h->bwd_block;
   cudaStream_t st = (cudaStream_t)stream;
   BwdArgs a;
   a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
@@ -779,17 +817,18 @@ static int vjp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   };
   const int slot = h->slot++ % Handle::RING;
   int *ctr = h->counters + 4 * slot;
-  a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
+  a.lsqr_iters = lsqr_iters; a.st = kernel_settings(*stg); a.counter = ctr + 1;
   // (values off chip: nothing of A is staged, use_tma only allows the bulk copy of P)
-  a.use_tma = h->bwd.vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = h->bwd.p_in_smem;
+  a.use_tma = gen.vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = gen.p_in_smem;
   CK(cudaSetDevice(h->device), "vjp set device");
-  a.ws = nullptr; a.ws_stride = (long long)h->bwd.ws_stride;
-  if (h->bwd.vec_global) {
-    if (!ensure_slab(h, &sw->bwd, nullptr, h->bwd.ws_stride * max_grid(h->bwd, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc backward workspace");
-    a.ws = sw->bwd;
+  a.ws = nullptr; a.ws_stride = (long long)gen.ws_stride;
+  if (gen.vec_global) {
+    double **slab = lsmr ? &sw->bwd_lsmr : &sw->bwd;
+    if (!ensure_slab(h, slab, nullptr, gen.ws_stride * max_grid(gen, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc backward workspace");
+    a.ws = *slab;
   }
   a.inst_list = nullptr; a.B_dev = nullptr; a.fail_list = nullptr; a.fail_count = nullptr; a.prof = h->prof;
-  if (h->block_bwd && stg->lsqr_precond == 2) {
+  if (block_bwd && stg->lsqr_precond == 2) {
     // pass 1: block-preconditioned solve; pass 2: equilibrated LSQR on the instances it rejected
     if (h->fail_cap[slot] < B) {
       int *p = nullptr;
@@ -799,18 +838,19 @@ static int vjp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
     CK(cudaMemsetAsync(ctr + 1, 0, 3 * sizeof(int), st), "vjp counters");
     h->last_block_slot = slot;
     a.fail_list = h->fail_list[slot]; a.fail_count = ctr + 2;
-    CK(launch(h->bwd_block, std::min(B, h->num_sms), &a, st), "vjp launch (block)");
+    CK(launch(bwd_block, std::min(B, h->num_sms), &a, st), "vjp launch (block)");
     BwdArgs f = a;
     f.st.lsqr_precond = 1; f.counter = ctr + 3; f.inst_list = h->fail_list[slot]; f.B_dev = ctr + 2;
     f.fail_list = nullptr; f.fail_count = nullptr;
-    CK(launch(h->bwd_fast, grid_for(h->bwd_fast, B, h->num_sms), &f, st), "vjp launch (fallback)");
+    const Plan &second = fast_bwd ? bwd_fast : pick(gen, B, h->num_sms, h->small_mode);   // (LSQR: always the fused kernel)
+    CK(launch(second, grid_for(second, B, h->num_sms), &f, st), "vjp launch (fallback)");
     h->launches += 2;
     return reduce();
   }
   if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // block factorisation not available for this structure
   CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "vjp counter");
-  const Plan &plan = h->fast_bwd ? h->bwd_fast : pick(h->bwd, B, h->num_sms, h->small_mode);
-  CK(launch(plan, grid_for(plan, B, h->num_sms), &a, st), h->fast_bwd ? "vjp launch (fast)" : "vjp launch");
+  const Plan &plan = fast_bwd ? bwd_fast : pick(gen, B, h->num_sms, h->small_mode);
+  CK(launch(plan, grid_for(plan, B, h->num_sms), &a, st), fast_bwd ? "vjp launch (fast)" : "vjp launch");
   h->launches++;
   return reduce();
 }
@@ -835,7 +875,10 @@ static int jvp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !dA_vals || !db || !dc || !dx || !dy || !stg)
     return fail(h, BCONE_EINVAL, "jvp: null argument");
   if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "jvp: structure has P but P_vals is NULL");
-  if (!h->jvp_ok) return fail(h, BCONE_EUNSUPPORTED, "jvp: the instance does not fit the generic LSQR kernel");
+  const bool lsmr = stg && stg->lsmr != 0;   // the LSQR or the LSMR kernel (settings.lsmr)
+  if (!lsmr && !h->jvp_ok) return fail(h, BCONE_EUNSUPPORTED, "jvp: the instance does not fit the generic LSQR kernel");
+  if (lsmr && !h->jvp_lsmr_ok) return fail(h, BCONE_EUNSUPPORTED, "jvp: the instance does not fit the generic LSMR kernel");
+  const TieredPlan &gen = lsmr ? h->jvp_lsmr : h->jvp;
   cudaStream_t st = (cudaStream_t)stream;
   BwdArgs a{};
   a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
@@ -843,19 +886,20 @@ static int jvp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   a.tA = dA_vals; a.tP = h->S.nnzP > 0 ? dP_vals : nullptr; a.tb = db; a.tc = dc; a.tx = dx; a.ty = dy; a.ts = ds;
   a.sA = shared ? 0 : h->S.nnzA; a.sP = shared ? 0 : h->S.nnzP;
   int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
-  a.lsqr_iters = lsqr_iters; a.st = *stg; a.counter = ctr + 1;
+  a.lsqr_iters = lsqr_iters; a.st = kernel_settings(*stg); a.counter = ctr + 1;
   if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // no block-preconditioned forward mode
-  a.use_tma = h->jvp.vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = h->jvp.p_in_smem;
+  a.use_tma = gen.vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = gen.p_in_smem;
   CK(cudaSetDevice(h->device), "jvp set device");
-  a.ws_stride = (long long)h->jvp.ws_stride;
-  if (h->jvp.vec_global) {
+  a.ws_stride = (long long)gen.ws_stride;
+  if (gen.vec_global) {
     Handle::StreamWs *sw = stream_ws(h, st);
-    if (!ensure_slab(h, &sw->jvp, nullptr, h->jvp.ws_stride * max_grid(h->jvp, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc jvp workspace");
-    a.ws = sw->jvp;
+    double **slab = lsmr ? &sw->jvp_lsmr : &sw->jvp;
+    if (!ensure_slab(h, slab, nullptr, gen.ws_stride * max_grid(gen, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc jvp workspace");
+    a.ws = *slab;
   }
   a.prof = h->prof;
   CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "jvp counter");
-  const Plan &plan = pick(h->jvp, B, h->num_sms, h->small_mode);
+  const Plan &plan = pick(gen, B, h->num_sms, h->small_mode);
   CK(launch(plan, grid_for(plan, B, h->num_sms), &a, st), "jvp launch");
   h->launches++;
   return BCONE_OK;

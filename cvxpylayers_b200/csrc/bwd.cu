@@ -18,23 +18,24 @@ struct BwdSmem {
   int *ibuf;
 };
 
-// v is only kept for the non-polyhedral rows (nonneg rows use pi_y > 0 <=> v > 0 as their mask).
-__host__ __device__ inline size_t bwd_vec_doubles(int n, int m, int npoly) {
+// v is only kept for the non-polyhedral rows (nonneg rows use pi_y > 0 <=> v > 0 as their mask).  LSMR keeps one more N-vector.
+__host__ __device__ inline size_t bwd_vec_doubles(int n, int m, int npoly, int lsmr = 0) {
   size_t N = (size_t)n + m + 1;
-  return 3 * (size_t)n + 2 * (size_t)m + (m - npoly) + 7 * N + 2 * (size_t)m;
+  return 3 * (size_t)n + 2 * (size_t)m + (m - npoly) + (lsmr ? 8 : 7) * N + 2 * (size_t)m;
 }
 // vec_global: large instances keep the LSQR vectors in a per-CTA slab of global memory.
 // vals_global: the CSR values are read in place from the caller's A_vals (instances whose values do not fit on chip).
 __host__ __device__ inline size_t bwd_smem_doubles(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
-                                                   int vals_global) {
+                                                   int vals_global, int lsmr = 0) {
   size_t d = 4 + (vals_global ? 0 : ((size_t)nnzA + 1) & ~(size_t)1) + (((size_t)nnzP_smem + 1) & ~(size_t)1) + threads + 2 * 32;
-  if (!vec_global) d += bwd_vec_doubles(n, m, npoly);
+  if (!vec_global) d += bwd_vec_doubles(n, m, npoly, lsmr);
   if (max_psd > 0) d += psd_total + (size_t)(threads / 32) * (3 * (size_t)max_psd * max_psd + max_psd);
   return d + 9 * (size_t)nexp;
 }
 
-// VG: no shared memory for the values (M.Av is set per instance)
-template <bool VG = false>
+// VG: no shared memory for the values (M.Av is set per instance); LSMR: one more N-vector behind t2 (LSMR's h-bar; not a
+// member of BwdSmem, whose layout the LSQR kernels' code depends on)
+template <bool VG = false, bool LSMR = false>
 __device__ __forceinline__ void carve_b(BwdSmem &M, double *base, double *gws, int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp) {
   const int N = n + m + 1;
   double *q = base;
@@ -51,6 +52,7 @@ __device__ __forceinline__ void carve_b(BwdSmem &M, double *base, double *gws, i
   M.U = v; v += N; M.V = v; v += N; M.W = v; v += N; M.X = v; v += N;
   M.Lsc = v; v += N; M.Rsc = v; v += N; M.tin = v; v += N;
   M.t1 = v; v += m; M.t2 = v; v += m;
+  if (LSMR) v += N;
   if (!gws) q = v;
   M.expJ = q; q += 9 * nexp;
   M.psdVL = q; q += psd_total;
@@ -307,14 +309,24 @@ __device__ __noinline__ void jvp_inactive_rows(const BwdArgs &a, const BwdSmem &
 // The adjoint's gradient assembly is G' and its dz is E'w, so it computes G' M^-T E'w; this computes E M^-1 G.
 // VG (values off chip): the instance's values are read in place from A_vals -- this kernel never writes them -- so nothing is
 // staged and shared memory holds only the vectors (when they fit) and the cone scratch.
+// LSMR: diffcp's mode = "lsmr" (settings.lsmr = 1) -- LSMR (common.cuh lsmr_block) in place of LSQR on the same operator,
+// scalings and right-hand side.  bwd_lsmr.cu compiles this file again with BC_LSMR defined: the same kernels with LSMR, named
+// bwd_lsmr_kernel, in a translation unit of their own (so that the LSQR kernels compile to the code they had without them).
+#ifdef BC_LSMR
+#define BWD_KERNEL bwd_lsmr_kernel
+constexpr bool LSMR = true;
+#else
+#define BWD_KERNEL bwd_kernel
+constexpr bool LSMR = false;
+#endif
 template <bool DENSE, bool SMALL = false, bool JVP = false, bool VG = false>   // SMALL: <= 256 threads, four resident CTAs per SM (see fwd.cu)
-__global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(const __grid_constant__ BwdArgs a) {
+__global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(const __grid_constant__ BwdArgs a) {
   extern __shared__ __align__(16) double smem[];
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, N = n + m + 1, T = blockDim.x, t = threadIdx.x;
-  const bcone_settings &st = a.st;
+  const bc_settings &st = a.st;
   BwdSmem M;
-  carve_b<VG>(M, smem, a.ws ? a.ws + (size_t)blockIdx.x * a.ws_stride : nullptr, n, m, S.z + S.l, S.nnzA, a.p_in_smem ? S.nnzP : 0, T, S.max_psd,
+  carve_b<VG, LSMR>(M, smem, a.ws ? a.ws + (size_t)blockIdx.x * a.ws_stride : nullptr, n, m, S.z + S.l, S.nnzA, a.p_in_smem ? S.nnzP : 0, T, S.max_psd,
               a.psd_total, S.ep + S.ed);
   if (t == 0) { mbar_init(M.bar, 1); fence_mbar_init(); }
   __syncthreads();
@@ -322,7 +334,14 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
   const ColPlan plA = make_colplan(m, n), plN = make_colplan(n, n);
 
   for (;;) {
-    if (t == 0) M.ibuf[0] = atomicAdd(a.counter, 1);
+    if constexpr (LSMR) {   // (also the second pass of the block-preconditioned LSMR adjoint: the instances on its device-side list)
+      if (t == 0) {
+        const int k = atomicAdd(a.counter, 1), nwork = a.B_dev ? *a.B_dev : a.B;
+        M.ibuf[0] = k < nwork ? (a.inst_list ? a.inst_list[k] : k) : a.B;
+      }
+    } else {
+      if (t == 0) M.ibuf[0] = atomicAdd(a.counter, 1);
+    }
     __syncthreads();
     const int inst = M.ibuf[0];
     if (inst >= a.B) break;
@@ -465,6 +484,25 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
         if constexpr (JVP) op_MT<DENSE>(a, M, Pg, xPx, src, out, pc ? Rs : nullptr, plA, plN);
         else op_M<DENSE>(a, M, Pg, xPx, src, out, pc ? Rs : nullptr, plA, plN);
       };
+#ifdef BC_LSMR   // (not if constexpr: a scope around the LSQR code below changes the code of the forward-mode kernels)
+      auto opB = [&](const double *in, double *out, double coef) {   // out <- B in + coef out, ||out||^2
+        for (int k = t; k < N; k += T) out[k] *= coef;
+        acc_B(in, out);
+        double q[1] = {0};
+        for (int k = t; k < N; k += T) q[0] = fma(out[k], out[k], q[0]);
+        block_reduce<1, false>(q, M.red);
+        return q[0];
+      };
+      auto opBT = [&](const double *in, double *out, double coef) {   // out <- B' in + coef out, ||out||^2
+        for (int k = t; k < N; k += T) out[k] *= coef;
+        acc_BT(in, out);
+        double q[1] = {0};
+        for (int k = t; k < N; k += T) q[0] = fma(out[k], out[k], q[0]);
+        block_reduce<1, false>(q, M.red);
+        return q[0];
+      };
+      itn = lsmr_block(N, M.U, M.V, M.W, M.t2 + m, M.X, M.red, st, iter_lim, opB, opBT);   // (u, v, h, h-bar, x)
+#else
       double r1[1] = {0};
       for (int k = t; k < N; k += T) r1[0] = fma(M.U[k], M.U[k], r1[0]);
       block_reduce<1, false>(r1, M.red);
@@ -536,6 +574,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
           if (istop) break;
         }
       }
+#endif
       if (pc) { __syncthreads(); for (int k = t; k < N; k += T) M.X[k] *= Rs[k]; }
       if constexpr (JVP) if (pc && S.l > 0) { __syncthreads(); jvp_inactive_rows<DENSE>(a, M, inst); }
     }
@@ -581,20 +620,28 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) bwd_kernel(c
   }
 }
 
-extern "C" size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
-                                    int vals_global) {
-  return bwd_smem_doubles(n, m, npoly, nnzA, nnzP_smem, threads, max_psd, psd_total, nexp, vec_global, vals_global) * sizeof(double);
-}
-extern "C" size_t bc_bwd_ws_doubles(int n, int m, int npoly) { return (bwd_vec_doubles(n, m, npoly) + 1) & ~(size_t)1; }
 // The instantiations that exist: the adjoint and the forward-mode derivative (same kernel, same shared-memory layout, JVP = true)
-// each as the 128-register build, the 4-CTA/SM build and the values-off-chip build (512-thread only).
+// each as the 128-register build, the 4-CTA/SM build and the values-off-chip build (512-thread only); each with LSQR
+// (bwd_kernel) and LSMR (bwd_lsmr_kernel).
 template <bool JVP>
 static const void *lsqr_kernel(int dense, int small_cta, int vals_global) {
   if (small_cta && vals_global) return nullptr;
-  if (vals_global) return dense ? (const void *)bwd_kernel<true, false, JVP, true> : (const void *)bwd_kernel<false, false, JVP, true>;
-  if (small_cta) return dense ? (const void *)bwd_kernel<true, true, JVP> : (const void *)bwd_kernel<false, true, JVP>;
-  return dense ? (const void *)bwd_kernel<true, false, JVP> : (const void *)bwd_kernel<false, false, JVP>;
+  if (vals_global) return dense ? (const void *)BWD_KERNEL<true, false, JVP, true> : (const void *)BWD_KERNEL<false, false, JVP, true>;
+  if (small_cta) return dense ? (const void *)BWD_KERNEL<true, true, JVP> : (const void *)BWD_KERNEL<false, true, JVP>;
+  return dense ? (const void *)BWD_KERNEL<true, false, JVP> : (const void *)BWD_KERNEL<false, false, JVP>;
 }
-extern "C" const void *bc_lsqr_kernel(int dense, int small_cta, int jvp, int vals_global) {
+#ifndef BC_LSMR
+extern "C" size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
+                                    int vals_global, int lsmr) {
+  return bwd_smem_doubles(n, m, npoly, nnzA, nnzP_smem, threads, max_psd, psd_total, nexp, vec_global, vals_global, lsmr) * sizeof(double);
+}
+extern "C" size_t bc_bwd_ws_doubles(int n, int m, int npoly, int lsmr) { return (bwd_vec_doubles(n, m, npoly, lsmr) + 1) & ~(size_t)1; }
+extern "C" const void *bc_lsqr_kernel(int dense, int small_cta, int jvp, int vals_global, int lsmr) {
+  if (lsmr) return bc_lsmr_kernel(dense, small_cta, jvp, vals_global);
   return jvp ? lsqr_kernel<true>(dense, small_cta, vals_global) : lsqr_kernel<false>(dense, small_cta, vals_global);
 }
+#else
+extern "C" const void *bc_lsmr_kernel(int dense, int small_cta, int jvp, int vals_global) {
+  return jvp ? lsqr_kernel<true>(dense, small_cta, vals_global) : lsqr_kernel<false>(dense, small_cta, vals_global);
+}
+#endif

@@ -43,12 +43,16 @@ __device__ __forceinline__ void carve_blk(BlkSmem &M, double *base, int n, int m
   M.live = (int *)q;
 }
 
-__global__ void __launch_bounds__(512, 1) bwd_block_kernel(const __grid_constant__ BwdArgs a) {
+// LSMR: diffcp's mode = "lsmr" (common.cuh lsmr_block) on the same preconditioned operator C, in the same shared memory (its
+// u starts on the right-hand side in place and h-bar takes LSQR's u); the kernel bwd_block_lsmr_kernel below.  The instances
+// it rejects go to an LSMR pass as well (api.cu).
+template <bool LSMR>
+__device__ __forceinline__ void bwd_block_body(const BwdArgs a) {   // (by value: by reference the LSQR kernel compiles to other code)
   extern __shared__ __align__(16) double smem[];
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, N = n + m + 1, T = blockDim.x, t = threadIdx.x;
   const int lane = t & 31, warp = t >> 5, nw = T >> 5;
-  const bcone_settings &st = a.st;
+  const bc_settings &st = a.st;
   BlkSmem M;
   carve_blk(M, smem, n, m, T);
   if (t == 0) { mbar_init(M.bar, 1); fence_mbar_init(); }
@@ -252,62 +256,66 @@ __global__ void __launch_bounds__(512, 1) bwd_block_kernel(const __grid_constant
         __syncthreads();
         return r2[0] + ot * ot;
       };
-      double r1[1] = {0};
-      for (int k = t; k < NR; k += T) { const double u = M.rhs[k]; M.U[k] = u; r1[0] = fma(u, u, r1[0]); M.V[k] = 0.0; }
-      block_reduce<1, false>(r1, M.red);
-      const double bnorm = sqrt(r1[0]);
-      double beta = bnorm, alfa = 0;
-      if (beta > 0) {
-        for (int k = t; k < NR; k += T) M.U[k] /= beta;
-        __syncthreads();
-        alfa = sqrt(CT_mul(M.U, M.V, 0.0));
-      }
-      if (alfa > 0) for (int k = t; k < NR; k += T) { const double v = M.V[k] / alfa; M.V[k] = v; M.W[k] = v; }
-      __syncthreads();
-      double rhobar = alfa, phibar = beta, anorm = 0, ddnorm = 0, xxnorm = 0, zz = 0, cs2 = -1, sn2 = 0;
-      if (alfa * beta != 0.0) {
-        while (itn < iter_lim) {
-          itn++;
-          beta = sqrt(C_mul(M.V, M.U, -alfa));
-          if (beta > 0) {
-            for (int k = t; k < NR; k += T) M.U[k] /= beta;
-            anorm = sqrt(anorm * anorm + alfa * alfa + beta * beta);
-            __syncthreads();
-            alfa = sqrt(CT_mul(M.U, M.V, -beta));
-            if (alfa > 0) for (int k = t; k < NR; k += T) M.V[k] /= alfa;
-          }
-          const double rho = hypot(rhobar, beta), cs = rhobar / rho, sn = beta / rho;
-          const double theta = sn * alfa;
-          rhobar = -cs * alfa;
-          const double phi = cs * phibar;
-          phibar = sn * phibar;
-          const double tau = sn * phi, t1c = phi / rho, t2c = -theta / rho;
+      if constexpr (LSMR) {
+        itn = lsmr_block(NR, M.rhs, M.V, M.W, M.U, M.z, M.red, st, iter_lim, C_mul, CT_mul);   // (u, v, h, h-bar, x)
+      } else {
+        double r1[1] = {0};
+        for (int k = t; k < NR; k += T) { const double u = M.rhs[k]; M.U[k] = u; r1[0] = fma(u, u, r1[0]); M.V[k] = 0.0; }
+        block_reduce<1, false>(r1, M.red);
+        const double bnorm = sqrt(r1[0]);
+        double beta = bnorm, alfa = 0;
+        if (beta > 0) {
+          for (int k = t; k < NR; k += T) M.U[k] /= beta;
           __syncthreads();
-          r1[0] = 0;
-          for (int k = t; k < NR; k += T) {
-            const double wk = M.W[k], dk = wk / rho;
-            r1[0] = fma(dk, dk, r1[0]);
-            M.z[k] = fma(t1c, wk, M.z[k]);
-            M.W[k] = fma(t2c, wk, M.V[k]);
+          alfa = sqrt(CT_mul(M.U, M.V, 0.0));
+        }
+        if (alfa > 0) for (int k = t; k < NR; k += T) { const double v = M.V[k] / alfa; M.V[k] = v; M.W[k] = v; }
+        __syncthreads();
+        double rhobar = alfa, phibar = beta, anorm = 0, ddnorm = 0, xxnorm = 0, zz = 0, cs2 = -1, sn2 = 0;
+        if (alfa * beta != 0.0) {
+          while (itn < iter_lim) {
+            itn++;
+            beta = sqrt(C_mul(M.V, M.U, -alfa));
+            if (beta > 0) {
+              for (int k = t; k < NR; k += T) M.U[k] /= beta;
+              anorm = sqrt(anorm * anorm + alfa * alfa + beta * beta);
+              __syncthreads();
+              alfa = sqrt(CT_mul(M.U, M.V, -beta));
+              if (alfa > 0) for (int k = t; k < NR; k += T) M.V[k] /= alfa;
+            }
+            const double rho = hypot(rhobar, beta), cs = rhobar / rho, sn = beta / rho;
+            const double theta = sn * alfa;
+            rhobar = -cs * alfa;
+            const double phi = cs * phibar;
+            phibar = sn * phibar;
+            const double tau = sn * phi, t1c = phi / rho, t2c = -theta / rho;
+            __syncthreads();
+            r1[0] = 0;
+            for (int k = t; k < NR; k += T) {
+              const double wk = M.W[k], dk = wk / rho;
+              r1[0] = fma(dk, dk, r1[0]);
+              M.z[k] = fma(t1c, wk, M.z[k]);
+              M.W[k] = fma(t2c, wk, M.V[k]);
+            }
+            block_reduce<1, false>(r1, M.red);
+            ddnorm += r1[0];
+            const double delta = sn2 * rho, gambar = -cs2 * rho, rhs_ = phi - delta * zz, zbar = rhs_ / gambar;
+            const double xnorm = sqrt(xxnorm + zbar * zbar);
+            const double gamma = hypot(gambar, theta);
+            cs2 = gambar / gamma; sn2 = theta / gamma; zz = rhs_ / gamma; xxnorm += zz * zz;
+            const double acond = anorm * sqrt(ddnorm), rnorm = phibar, arnorm = alfa * fabs(tau);
+            const double test1 = rnorm / bnorm, test2 = arnorm / (anorm * rnorm + eps), test3 = 1.0 / (acond + eps);
+            const double tt1 = test1 / (1.0 + anorm * xnorm / bnorm), rtol = btol + atol * anorm * xnorm / bnorm;
+            int istop = 0;
+            if (itn >= iter_lim) istop = 7;
+            if (1.0 + test3 <= 1.0) istop = 6;
+            if (1.0 + test2 <= 1.0) istop = 5;
+            if (1.0 + tt1 <= 1.0) istop = 4;
+            if (test3 <= ctol) istop = 3;
+            if (test2 <= atol) istop = 2;
+            if (test1 <= rtol) istop = 1;
+            if (istop) break;
           }
-          block_reduce<1, false>(r1, M.red);
-          ddnorm += r1[0];
-          const double delta = sn2 * rho, gambar = -cs2 * rho, rhs_ = phi - delta * zz, zbar = rhs_ / gambar;
-          const double xnorm = sqrt(xxnorm + zbar * zbar);
-          const double gamma = hypot(gambar, theta);
-          cs2 = gambar / gamma; sn2 = theta / gamma; zz = rhs_ / gamma; xxnorm += zz * zz;
-          const double acond = anorm * sqrt(ddnorm), rnorm = phibar, arnorm = alfa * fabs(tau);
-          const double test1 = rnorm / bnorm, test2 = arnorm / (anorm * rnorm + eps), test3 = 1.0 / (acond + eps);
-          const double tt1 = test1 / (1.0 + anorm * xnorm / bnorm), rtol = btol + atol * anorm * xnorm / bnorm;
-          int istop = 0;
-          if (itn >= iter_lim) istop = 7;
-          if (1.0 + test3 <= 1.0) istop = 6;
-          if (1.0 + test2 <= 1.0) istop = 5;
-          if (1.0 + tt1 <= 1.0) istop = 4;
-          if (test3 <= ctol) istop = 3;
-          if (test2 <= atol) istop = 2;
-          if (test1 <= rtol) istop = 1;
-          if (istop) break;
         }
       }
     }
@@ -353,5 +361,14 @@ __global__ void __launch_bounds__(512, 1) bwd_block_kernel(const __grid_constant
   }
 }
 
+#ifndef BC_LSMR
+__global__ void __launch_bounds__(512, 1) bwd_block_kernel(const __grid_constant__ BwdArgs a) { bwd_block_body<false>(a); }
+
 extern "C" size_t bc_bwdb_smem_bytes(int n, int m, int threads) { return bwdb_smem_doubles(n, m, threads) * sizeof(double); }
-extern "C" const void *bc_bwdb_kernel(void) { return (const void *)bwd_block_kernel; }
+extern "C" const void *bc_bwdb_kernel(int lsmr) { return lsmr ? bc_bwdb_lsmr_kernel() : (const void *)bwd_block_kernel; }
+#else
+// bwd_block_lsmr.cu: the LSMR kernel, in a translation unit of its own (next to it the LSQR kernel compiles to other code)
+__global__ void __launch_bounds__(512, 1) bwd_block_lsmr_kernel(const __grid_constant__ BwdArgs a) { bwd_block_body<true>(a); }
+
+extern "C" const void *bc_bwdb_lsmr_kernel(void) { return (const void *)bwd_block_lsmr_kernel; }
+#endif

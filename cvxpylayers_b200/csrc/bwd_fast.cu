@@ -17,18 +17,21 @@
 
 struct FastSmem {
   double *Av, *Pv, *x, *c, *px2c, *piy, *b, *U, *V, *W, *X, *Lsc, *Rsc, *ein, *prow, *part, *red;
+  double *Hb;   // LSMR only: its h-bar (U, V, W, X are u, v, h, x)
   int *rows;
   uint64_t *bar;
   int *ibuf;
 };
 
-__host__ __device__ inline size_t bwdf_smem_doubles(int n, int m, int nnzA, int nnzP, int threads) {
+// lsmr: the LSMR variant keeps one more N-vector
+__host__ __device__ inline size_t bwdf_smem_doubles(int n, int m, int nnzA, int nnzP, int threads, int lsmr = 0) {
   const size_t N = (size_t)n + m + 1;
   const size_t part = (size_t)8 * n > (size_t)threads ? (size_t)8 * n : (size_t)threads;
-  return 4 + (((size_t)nnzA + 1) & ~(size_t)1) + (((size_t)nnzP + 1) & ~(size_t)1) + 3 * (size_t)n + 2 * (size_t)m + 6 * N + ((N + 1) & ~(size_t)1) + n + part +
-         3 * 32 + ((size_t)m + n + 2) / 2 + 4;
+  return 4 + (((size_t)nnzA + 1) & ~(size_t)1) + (((size_t)nnzP + 1) & ~(size_t)1) + 3 * (size_t)n + 2 * (size_t)m + (lsmr ? 7 : 6) * N + ((N + 1) & ~(size_t)1) + n +
+         part + 3 * 32 + ((size_t)m + n + 2) / 2 + 4;
 }
 
+template <bool LSMR = false>
 __device__ __forceinline__ void carve_f(FastSmem &M, double *base, int n, int m, int nnzA, int nnzP, int threads) {
   const int N = n + m + 1;
   double *q = base;
@@ -41,6 +44,7 @@ __device__ __forceinline__ void carve_f(FastSmem &M, double *base, int n, int m,
   M.x = q; q += n; M.c = q; q += n; M.px2c = q; q += n;
   M.piy = q; q += m; M.b = q; q += m;
   M.U = q; q += N; M.V = q; q += N; M.W = q; q += N; M.X = q; q += N; M.Lsc = q; q += N; M.Rsc = q; q += N;
+  if (LSMR) { M.Hb = q; q += N; }
   M.prow = q; q += n;
   M.red = q; q += 3 * 32;
   M.rows = (int *)q;
@@ -184,14 +188,16 @@ __device__ __forceinline__ double fast_op(const FastSmem &M, const DevStruct &S,
   return r3[1] + ot * ot;
 }
 
-template <int NCH>
-__global__ void __launch_bounds__(512, 1) bwd_fast_kernel(const __grid_constant__ BwdArgs a) {
+// LSMR: diffcp's mode = "lsmr" (common.cuh lsmr_block) on the same operator, scalings and right-hand side; the kernel
+// bwd_fast_lsmr_kernel below.
+template <int NCH, bool LSMR>
+__device__ __forceinline__ void bwd_fast_body(const BwdArgs &a) {   // (by reference: by value the LSQR kernels compile to other code)
   extern __shared__ __align__(16) double smem[];
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, N = n + m + 1, T = blockDim.x, t = threadIdx.x;
-  const bcone_settings &st = a.st;
+  const bc_settings &st = a.st;
   FastSmem M;
-  carve_f(M, smem, n, m, S.nnzA, S.nnzP, T);
+  carve_f<LSMR>(M, smem, n, m, S.nnzA, S.nnzP, T);
   if (t == 0) { mbar_init(M.bar, 1); fence_mbar_init(); }
   __syncthreads();
   uint32_t tma_phase = 0;
@@ -326,75 +332,93 @@ __global__ void __launch_bounds__(512, 1) bwd_fast_kernel(const __grid_constant_
         __syncthreads();
       }
       const double *Ls = pc ? M.Lsc : nullptr, *Rs = pc ? M.Rsc : nullptr;
-      // ---- LSQR on B = diag(L) M' diag(R); u, v stored un-normalised (u = U/beta, v = V/alfa) ----
-      const double eps = 2.220446049250313e-16;
-      const double atol = st.lsqr_atol, btol = st.lsqr_btol;
-      const double ctol = st.lsqr_conlim > 0 ? 1.0 / st.lsqr_conlim : 0.0;
-      const int iter_lim = st.lsqr_iter_lim < 0 ? 2 * N : st.lsqr_iter_lim;
-      double r1[1] = {0};
-      for (int k = t; k < N; k += T) { r1[0] = fma(M.U[k], M.U[k], r1[0]); M.V[k] = 0.0; }
-      block_reduce<1, false>(r1, M.red);
-      const double bnorm = sqrt(r1[0]), ibnorm = bnorm > 0 ? 1.0 / bnorm : 0.0;
-      double beta = bnorm, alfa = 0, wn2 = 0;
-      if (beta > 0) {
-        __syncthreads();
-        alfa = sqrt(fast_op<false, NCH>(M, S, nlist, xPx, M.U, Ls, 1.0 / beta, M.V, Rs, 0.0, wn2));   // V = B' u
-        __syncthreads();
-      }
-      if (alfa > 0) for (int k = t; k < N; k += T) M.W[k] = M.V[k] / alfa;
-      wn2 = (t == 0) ? 1.0 : 0.0;  // ||w_1||^2 = ||v_1||^2 = 1, carried through the next block reduction
-      __syncthreads();
-      double rhobar = alfa, phibar = beta, anorm = 0, ddnorm = 0, xxnorm = 0, z = 0, cs2 = -1, sn2 = 0;
-      if (alfa * beta != 0.0) {
-        while (itn < iter_lim) {
-          itn++;
-          // U = B v - alfa u
-          const double nb2 = fast_op<true, NCH>(M, S, nlist, xPx, M.V, Rs, 1.0 / alfa, M.U, Ls, -alfa / beta, wn2);
-          const double wnorm2 = wn2;   // ||w_k||^2 of the current w
-          beta = sqrt(nb2);
+      if constexpr (LSMR) {
+        // ---- LSMR on B = diag(L) M' diag(R); u, v normalised ----
+        const int iter_lim = st.lsqr_iter_lim < 0 ? 2 * N : st.lsqr_iter_lim;
+        auto opB = [&](const double *in, double *out, double coef) {   // out <- B in + coef out, ||out||^2
+          double dummy = 0;
+          const double r = fast_op<true, NCH>(M, S, nlist, xPx, in, Rs, 1.0, out, Ls, coef, dummy);
           __syncthreads();
-          if (beta > 0) {
-            anorm = sqrt(anorm * anorm + alfa * alfa + beta * beta);
-            double dummy = 0;
-            const double na2 = fast_op<false, NCH>(M, S, nlist, xPx, M.U, Ls, 1.0 / beta, M.V, Rs, -beta / alfa, dummy);  // V = B' u - beta v
-            alfa = sqrt(na2);
+          return r;
+        };
+        auto opBT = [&](const double *in, double *out, double coef) {   // out <- B' in + coef out, ||out||^2
+          double dummy = 0;
+          const double r = fast_op<false, NCH>(M, S, nlist, xPx, in, Ls, 1.0, out, Rs, coef, dummy);
+          __syncthreads();
+          return r;
+        };
+        itn = lsmr_block(N, M.U, M.V, M.W, M.Hb, M.X, M.red, st, iter_lim, opB, opBT);   // (u, v, h, h-bar, x)
+      } else {
+        // ---- LSQR on B = diag(L) M' diag(R); u, v stored un-normalised (u = U/beta, v = V/alfa) ----
+        const double eps = 2.220446049250313e-16;
+        const double atol = st.lsqr_atol, btol = st.lsqr_btol;
+        const double ctol = st.lsqr_conlim > 0 ? 1.0 / st.lsqr_conlim : 0.0;
+        const int iter_lim = st.lsqr_iter_lim < 0 ? 2 * N : st.lsqr_iter_lim;
+        double r1[1] = {0};
+        for (int k = t; k < N; k += T) { r1[0] = fma(M.U[k], M.U[k], r1[0]); M.V[k] = 0.0; }
+        block_reduce<1, false>(r1, M.red);
+        const double bnorm = sqrt(r1[0]), ibnorm = bnorm > 0 ? 1.0 / bnorm : 0.0;
+        double beta = bnorm, alfa = 0, wn2 = 0;
+        if (beta > 0) {
+          __syncthreads();
+          alfa = sqrt(fast_op<false, NCH>(M, S, nlist, xPx, M.U, Ls, 1.0 / beta, M.V, Rs, 0.0, wn2));   // V = B' u
+          __syncthreads();
+        }
+        if (alfa > 0) for (int k = t; k < N; k += T) M.W[k] = M.V[k] / alfa;
+        wn2 = (t == 0) ? 1.0 : 0.0;  // ||w_1||^2 = ||v_1||^2 = 1, carried through the next block reduction
+        __syncthreads();
+        double rhobar = alfa, phibar = beta, anorm = 0, ddnorm = 0, xxnorm = 0, z = 0, cs2 = -1, sn2 = 0;
+        if (alfa * beta != 0.0) {
+          while (itn < iter_lim) {
+            itn++;
+            // U = B v - alfa u
+            const double nb2 = fast_op<true, NCH>(M, S, nlist, xPx, M.V, Rs, 1.0 / alfa, M.U, Ls, -alfa / beta, wn2);
+            const double wnorm2 = wn2;   // ||w_k||^2 of the current w
+            beta = sqrt(nb2);
             __syncthreads();
+            if (beta > 0) {
+              anorm = sqrt(anorm * anorm + alfa * alfa + beta * beta);
+              double dummy = 0;
+              const double na2 = fast_op<false, NCH>(M, S, nlist, xPx, M.U, Ls, 1.0 / beta, M.V, Rs, -beta / alfa, dummy);  // V = B' u - beta v
+              alfa = sqrt(na2);
+              __syncthreads();
+            }
+            // scalar recurrences of LSQR (same quantities as SciPy's; reciprocals shared, stopping
+            // ratios compared by cross-multiplication to keep fp64 divisions off the critical path)
+            const double rho = sqrt(fma(rhobar, rhobar, beta * beta)), irho = 1.0 / rho;
+            const double cs = rhobar * irho, sn = beta * irho;
+            const double theta = sn * alfa;
+            rhobar = -cs * alfa;
+            const double phi = cs * phibar;
+            phibar = sn * phibar;
+            const double tau = sn * phi;
+            const double t1c = phi * irho, t2c = -theta * irho, ialfa = alfa > 0 ? 1.0 / alfa : 0.0;
+            wn2 = 0;
+            for (int k = t; k < N; k += T) {
+              const double wk = M.W[k];
+              M.X[k] = fma(t1c, wk, M.X[k]);
+              const double wnew = fma(t2c, wk, M.V[k] * ialfa);
+              M.W[k] = wnew; wn2 = fma(wnew, wnew, wn2);
+            }
+            ddnorm = fma(wnorm2, irho * irho, ddnorm);
+            const double delta = sn2 * rho, gambar = -cs2 * rho, rhs = phi - delta * z, zbar = rhs / gambar;
+            const double xnorm = sqrt(fma(zbar, zbar, xxnorm));
+            const double gamma = sqrt(fma(gambar, gambar, theta * theta)), igamma = 1.0 / gamma;
+            cs2 = gambar * igamma; sn2 = theta * igamma; z = rhs * igamma; xxnorm = fma(z, z, xxnorm);
+            const double acond = anorm * sqrt(ddnorm), rnorm = phibar, arnorm = alfa * fabs(tau);
+            const double test1 = rnorm * ibnorm, den2 = fma(anorm, rnorm, eps), den3 = acond + eps;
+            const double axb = anorm * xnorm * ibnorm, rtol = fma(atol, axb, btol);
+            const double u = 1.1102230246251565e-16;   // 1 + t <= 1  <=>  t <= 2^-53
+            int istop = 0;
+            if (itn >= iter_lim) istop = 7;
+            if (1.0 <= u * den3) istop = 6;
+            if (arnorm <= u * den2) istop = 5;
+            if (test1 <= u * (1.0 + axb)) istop = 4;
+            if (1.0 <= ctol * den3) istop = 3;
+            if (arnorm <= atol * den2) istop = 2;
+            if (test1 <= rtol) istop = 1;
+            if (istop || !(alfa > 0) || !(beta > 0)) break;
           }
-          // scalar recurrences of LSQR (same quantities as SciPy's; reciprocals shared, stopping
-          // ratios compared by cross-multiplication to keep fp64 divisions off the critical path)
-          const double rho = sqrt(fma(rhobar, rhobar, beta * beta)), irho = 1.0 / rho;
-          const double cs = rhobar * irho, sn = beta * irho;
-          const double theta = sn * alfa;
-          rhobar = -cs * alfa;
-          const double phi = cs * phibar;
-          phibar = sn * phibar;
-          const double tau = sn * phi;
-          const double t1c = phi * irho, t2c = -theta * irho, ialfa = alfa > 0 ? 1.0 / alfa : 0.0;
-          wn2 = 0;
-          for (int k = t; k < N; k += T) {
-            const double wk = M.W[k];
-            M.X[k] = fma(t1c, wk, M.X[k]);
-            const double wnew = fma(t2c, wk, M.V[k] * ialfa);
-            M.W[k] = wnew; wn2 = fma(wnew, wnew, wn2);
-          }
-          ddnorm = fma(wnorm2, irho * irho, ddnorm);
-          const double delta = sn2 * rho, gambar = -cs2 * rho, rhs = phi - delta * z, zbar = rhs / gambar;
-          const double xnorm = sqrt(fma(zbar, zbar, xxnorm));
-          const double gamma = sqrt(fma(gambar, gambar, theta * theta)), igamma = 1.0 / gamma;
-          cs2 = gambar * igamma; sn2 = theta * igamma; z = rhs * igamma; xxnorm = fma(z, z, xxnorm);
-          const double acond = anorm * sqrt(ddnorm), rnorm = phibar, arnorm = alfa * fabs(tau);
-          const double test1 = rnorm * ibnorm, den2 = fma(anorm, rnorm, eps), den3 = acond + eps;
-          const double axb = anorm * xnorm * ibnorm, rtol = fma(atol, axb, btol);
-          const double u = 1.1102230246251565e-16;   // 1 + t <= 1  <=>  t <= 2^-53
-          int istop = 0;
-          if (itn >= iter_lim) istop = 7;
-          if (1.0 <= u * den3) istop = 6;
-          if (arnorm <= u * den2) istop = 5;
-          if (test1 <= u * (1.0 + axb)) istop = 4;
-          if (1.0 <= ctol * den3) istop = 3;
-          if (arnorm <= atol * den2) istop = 2;
-          if (test1 <= rtol) istop = 1;
-          if (istop || !(alfa > 0) || !(beta > 0)) break;
         }
       }
       __syncthreads();
@@ -428,7 +452,21 @@ __global__ void __launch_bounds__(512, 1) bwd_fast_kernel(const __grid_constant_
   }
 }
 
-extern "C" size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads) {
-  return bwdf_smem_doubles(n, m, nnzA, nnzP, threads) * sizeof(double);
+#ifndef BC_LSMR
+template <int NCH>
+__global__ void __launch_bounds__(512, 1) bwd_fast_kernel(const __grid_constant__ BwdArgs a) { bwd_fast_body<NCH, false>(a); }
+
+extern "C" size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads, int lsmr) {
+  return bwdf_smem_doubles(n, m, nnzA, nnzP, threads, lsmr) * sizeof(double);
 }
-extern "C" const void *bc_bwdf_kernel(int n) { return n <= 64 ? (const void *)bwd_fast_kernel<1> : (const void *)bwd_fast_kernel<2>; }
+extern "C" const void *bc_bwdf_kernel(int n, int lsmr) {
+  if (lsmr) return bc_bwdf_lsmr_kernel(n);
+  return n <= 64 ? (const void *)bwd_fast_kernel<1> : (const void *)bwd_fast_kernel<2>;
+}
+#else
+// bwd_fast_lsmr.cu: the LSMR kernels, in a translation unit of their own (next to them the LSQR kernels compile to other code)
+template <int NCH>
+__global__ void __launch_bounds__(512, 1) bwd_fast_lsmr_kernel(const __grid_constant__ BwdArgs a) { bwd_fast_body<NCH, true>(a); }
+
+extern "C" const void *bc_bwdf_lsmr_kernel(int n) { return n <= 64 ? (const void *)bwd_fast_lsmr_kernel<1> : (const void *)bwd_fast_lsmr_kernel<2>; }
+#endif

@@ -9,6 +9,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stddef.h>
 #include "../../include/bcone.h"
 
 #define BC_TAU_FACTOR 10.0
@@ -38,6 +39,22 @@ struct DevStruct {
   const int *cone_type, *cone_start, *cone_size, *cone_order; // [ncones], rows are offsets in y
 };
 
+// The settings the kernels read: bcone_settings without its trailing lsmr field, which the host turns into the choice of
+// kernel (so the argument blocks below keep their layout, and the LSQR kernels their code).  Field for field the same.
+struct bc_settings {
+  double eps_abs, eps_rel, eps_infeas, alpha, rho_x, scale, lsqr_atol, lsqr_btol, lsqr_conlim;
+  int32_t max_iters, normalize, adaptive_scale, check_interval, ruiz_passes, lsqr_iter_lim, lsqr_precond, adaptive_check;
+  int32_t acceleration_lookback, acceleration_interval;
+};
+static_assert(sizeof(bc_settings) == offsetof(bcone_settings, lsmr) && offsetof(bc_settings, lsqr_conlim) == offsetof(bcone_settings, lsqr_conlim) &&
+                  offsetof(bc_settings, acceleration_interval) == offsetof(bcone_settings, acceleration_interval),
+              "bc_settings must be bcone_settings up to its lsmr field");
+inline bc_settings kernel_settings(const bcone_settings &s) {
+  return {s.eps_abs, s.eps_rel, s.eps_infeas, s.alpha, s.rho_x, s.scale, s.lsqr_atol, s.lsqr_btol, s.lsqr_conlim,
+          s.max_iters, s.normalize, s.adaptive_scale, s.check_interval, s.ruiz_passes, s.lsqr_iter_lim, s.lsqr_precond, s.adaptive_check,
+          s.acceleration_lookback, s.acceleration_interval};
+}
+
 // Kernel argument blocks (passed by value as __grid_constant__).
 struct FwdArgs {
   DevStruct S;
@@ -46,7 +63,7 @@ struct FwdArgs {
   double *x, *y, *s;
   int *status, *iters;
   double *resid;
-  bcone_settings st;
+  bc_settings st;
   int *counter;
   int use_tma;
   double *ws;            // INDIRECT mode: per-CTA slab of global memory holding the iterate vectors
@@ -74,7 +91,7 @@ struct BwdArgs {
   const double *A_vals, *P_vals, *b, *c, *x, *y, *s, *dx, *dy;
   double *dA, *dP, *db, *dc;
   int *lsqr_iters;
-  bcone_settings st;
+  bc_settings st;
   int *counter;
   int use_tma;
   int psd_total;  // sum over PSD blocks of k^2 + k
@@ -1459,6 +1476,119 @@ __device__ __forceinline__ void project_cones(const DevStruct &S, double *v, dou
   }
 }
 
+// ----------------------------------------------------------------------------- LSMR
+// The adjoint / forward-mode least-squares solve with diffcp's mode = "lsmr": LSMR (Fong & Saunders 2011) with the recurrences,
+// norm / condition estimates and stopping rules of scipy.sparse.linalg.lsmr at damp = 0 (SciPy's rotation Qhat is then
+// (sign(alphabar), 0, |alphabar|)).  Shared by the three backward kernels, which differ only in the operator.
+
+// SciPy's _sym_ortho: the stable Givens rotation [c s; -s c] [a; b] = [r; 0]
+__device__ __forceinline__ void sym_ortho(double a, double b, double &c, double &s, double &r) {
+  if (b == 0) { c = a > 0 ? 1.0 : (a < 0 ? -1.0 : 0.0); s = 0.0; r = fabs(a); }
+  else if (a == 0) { c = 0.0; s = b > 0 ? 1.0 : -1.0; r = fabs(b); }
+  else if (fabs(b) > fabs(a)) { const double tau = a / b; s = copysign(1.0, b) / sqrt(1.0 + tau * tau); c = s * tau; r = b / s; }
+  else { const double tau = b / a; c = copysign(1.0, a) / sqrt(1.0 + tau * tau); s = c * tau; r = a / c; }
+}
+
+// Block-cooperative LSMR on an N x N operator B: every thread of the block calls it with the same arguments.  U holds the
+// right-hand side on entry; V, H, Hb are work vectors; X returns the solution (B'B X = B' rhs in the least-squares sense).
+// opB(in, out, coef): out <- B in + coef out, opBT the same with B'; both return ||out||^2 (the same bits in every thread)
+// and end with a barrier.  Returns the iteration count (0: b = 0 or B'b = 0, X = 0).
+template <class OpB, class OpBT>
+__device__ __forceinline__ int lsmr_block(int N, double *U, double *V, double *H, double *Hb, double *X, double *red, const bc_settings &st,
+                                       int iter_lim, OpB opB, OpBT opBT) {
+  const int t = threadIdx.x, T = blockDim.x;
+  const double atol = st.lsqr_atol, btol = st.lsqr_btol, ctol = st.lsqr_conlim > 0 ? 1.0 / st.lsqr_conlim : 0.0;
+  double r1[1] = {0};
+  for (int k = t; k < N; k += T) { r1[0] = fma(U[k], U[k], r1[0]); X[k] = 0.0; V[k] = 0.0; }
+  block_reduce<1, false>(r1, red);
+  const double normb = sqrt(r1[0]);
+  double beta = normb, alpha = 0;
+  if (beta > 0) {
+    const double ib = 1.0 / beta;
+    for (int k = t; k < N; k += T) U[k] *= ib;
+    __syncthreads();
+    alpha = sqrt(opBT(U, V, 0.0));   // v = B' u
+  }
+  {
+    const double ia = alpha > 0 ? 1.0 / alpha : 1.0;
+    for (int k = t; k < N; k += T) { const double v = V[k] * ia; V[k] = v; H[k] = v; Hb[k] = 0.0; }
+    __syncthreads();
+  }
+  if (alpha * beta == 0.0) return 0;   // SciPy: normar = alpha beta = 0 or normb = 0 -> x = 0
+  double zetabar = alpha * beta, alphabar = alpha, rho = 1, rhobar = 1, cbar = 1, sbar = 0;
+  double betadd = beta, betad = 0, rhodold = 1, tautildeold = 0, thetatilde = 0, zeta = 0, d = 0;
+  double normA2 = alpha * alpha, maxrbar = 0, minrbar = 1e100;
+  int itn = 0;
+  while (itn < iter_lim) {
+    itn++;
+    beta = sqrt(opB(V, U, -alpha));   // u = B v - alpha u
+    double vs = 1.0;                    // v's normalisation, applied in the update pass below
+    if (beta > 0) {
+      const double ib = 1.0 / beta;
+      for (int k = t; k < N; k += T) U[k] *= ib;
+      __syncthreads();
+      alpha = sqrt(opBT(U, V, -beta));   // v = B' u - beta v
+      if (alpha > 0) vs = 1.0 / alpha;
+    }
+    double chat, shat, alphahat;
+    sym_ortho(alphabar, 0.0, chat, shat, alphahat);
+    const double rhoold = rho;
+    double c, s;
+    sym_ortho(alphahat, beta, c, s, rho);
+    const double thetanew = s * alpha;
+    alphabar = c * alpha;
+    const double rhobarold = rhobar, zetaold = zeta, thetabar = sbar * rho, rhotemp = cbar * rho;
+    sym_ortho(cbar * rho, thetanew, cbar, sbar, rhobar);
+    zeta = cbar * zetabar;
+    zetabar = -sbar * zetabar;
+    // hbar = h - thetabar rho / (rhoold rhobarold) hbar;  x += zeta / (rho rhobar) hbar;  h = v - thetanew / rho h;  ||x||^2
+    const double chb = -(thetabar * rho / (rhoold * rhobarold)), cx = zeta / (rho * rhobar), ch = -(thetanew / rho);
+    r1[0] = 0;
+    for (int k = t; k < N; k += T) {
+      const double v = V[k] * vs, h = H[k];
+      const double hb = fma(Hb[k], chb, h), x = fma(cx, hb, X[k]);
+      V[k] = v; Hb[k] = hb; X[k] = x; H[k] = fma(h, ch, v);
+      r1[0] = fma(x, x, r1[0]);
+    }
+    block_reduce<1, false>(r1, red);
+    const double normx = sqrt(r1[0]);
+    // ||r|| estimate
+    const double betaacute = chat * betadd, betacheck = -shat * betadd, betahat = c * betaacute;
+    betadd = -s * betaacute;
+    const double thetatildeold = thetatilde;
+    double ctildeold, stildeold, rhotildeold;
+    sym_ortho(rhodold, thetabar, ctildeold, stildeold, rhotildeold);
+    thetatilde = stildeold * rhobar;
+    rhodold = ctildeold * rhobar;
+    betad = -stildeold * betad + ctildeold * betahat;
+    tautildeold = (zetaold - thetatildeold * tautildeold) / rhotildeold;
+    const double taud = (zeta - thetatilde * tautildeold) / rhodold;
+    d += betacheck * betacheck;
+    const double normr = sqrt(d + (betad - taud) * (betad - taud) + betadd * betadd);
+    // ||B|| and cond(B) estimates
+    normA2 += beta * beta;
+    const double normA = sqrt(normA2);
+    normA2 += alpha * alpha;
+    maxrbar = fmax(maxrbar, rhobarold);
+    if (itn > 1) minrbar = fmin(minrbar, rhobarold);
+    const double condA = fmax(maxrbar, rhotemp) / fmin(minrbar, rhotemp);
+    // stopping rules
+    const double normar = fabs(zetabar);
+    const double test1 = normr / normb, test2 = normA * normr != 0.0 ? normar / (normA * normr) : INFINITY, test3 = 1.0 / condA;
+    const double t1 = test1 / (1.0 + normA * normx / normb), rtol = btol + atol * normA * normx / normb;
+    int istop = 0;
+    if (itn >= iter_lim) istop = 7;
+    if (1.0 + test3 <= 1.0) istop = 6;
+    if (1.0 + test2 <= 1.0) istop = 5;
+    if (1.0 + t1 <= 1.0) istop = 4;
+    if (test3 <= ctol) istop = 3;
+    if (test2 <= atol) istop = 2;
+    if (test1 <= rtol) istop = 1;
+    if (istop) break;
+  }
+  return itn;
+}
+
 // ----------------------------------------------------------------------------- host entry points
 // Everything api.cu calls in the kernel files, declared once so that the compiler checks each definition against its uses.
 // Per kernel family: the size functions, and one lookup from the variant to the kernel's address (nullptr: no such
@@ -1475,16 +1605,20 @@ int bc_fwdf_threads(void);
 size_t bc_fwdf_cache_doubles(int n, int m);
 int bc_fwdf_eligible(int n, int m);
 const void *bc_fwdf_kernel(int n, int m);
-// bwd.cu (adjoint and forward mode)
+// bwd.cu (adjoint and forward mode; lsmr: the LSMR variant, one more N-vector)
 size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
-                         int vals_global);
-size_t bc_bwd_ws_doubles(int n, int m, int npoly);
-const void *bc_lsqr_kernel(int dense, int small_cta, int jvp, int vals_global);
+                         int vals_global, int lsmr);
+size_t bc_bwd_ws_doubles(int n, int m, int npoly, int lsmr);
+const void *bc_lsqr_kernel(int dense, int small_cta, int jvp, int vals_global, int lsmr);
 // bwd_fast.cu, bwd_block.cu
-size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads);
-const void *bc_bwdf_kernel(int n);
-size_t bc_bwdb_smem_bytes(int n, int m, int threads);
-const void *bc_bwdb_kernel(void);
+size_t bc_bwdf_smem_bytes(int n, int m, int nnzA, int nnzP, int threads, int lsmr);
+const void *bc_bwdf_kernel(int n, int lsmr);
+size_t bc_bwdb_smem_bytes(int n, int m, int threads);   // (the same for both variants)
+const void *bc_bwdb_kernel(int lsmr);
+// bwd_lsmr.cu, bwd_fast_lsmr.cu, bwd_block_lsmr.cu: the LSMR kernels (reached through the three lookups above)
+const void *bc_lsmr_kernel(int dense, int small_cta, int jvp, int vals_global);
+const void *bc_bwdf_lsmr_kernel(int n);
+const void *bc_bwdb_lsmr_kernel(void);
 // pack.cu
 cudaError_t bc_b2e(const double *in, double *out, int K, int B, int ldo, int roff, const int *smap, const int *dmap, double sign, long long ldb,
                    cudaStream_t st);

@@ -271,7 +271,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) fwd_kernel(c
   extern __shared__ __align__(16) double smem[];
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, N = n + m + 1, T = blockDim.x, t = threadIdx.x;
-  const bcone_settings &st = a.st;
+  const bc_settings &st = a.st;
   FwdSmem M;
   if constexpr (VG) {
     double *const slab = a.ws + (size_t)blockIdx.x * a.ws_stride;   // [values (even count: 16-byte aligned) | vectors | factor]

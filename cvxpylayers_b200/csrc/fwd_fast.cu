@@ -382,7 +382,7 @@ enum { SC_SIGMA = 0, SC_NB0, SC_NC0, SC_SUMLOG, SC_PREVLR, SC_RP, SC_RD, SC_GAP,
 __device__ __noinline__ void check_tail(const FwdArgs &a, double *vx, double *vy, double *red, double *scratch, const double *Pv,
                                         int npad, int mpad, int it, double scale, double tau) {
   const DevStruct &S = a.S;
-  const bcone_settings &st = a.st;
+  const bc_settings &st = a.st;
   const int n = S.n, m = S.m, t = threadIdx.x, z = S.z;
   double *sc = red + 256;
   const double *ux = vx + npad, *ch = vx + 4 * npad, *En = vx + 5 * npad, *tn = vx + 6 * npad;
@@ -584,7 +584,7 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
   extern __shared__ __align__(16) double sm[];
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, t = threadIdx.x, z = S.z;
-  const bcone_settings &st = a.st;
+  const bc_settings &st = a.st;
   const Geo<CT_, RTU_> g(n, m);
   uint64_t *bar = (uint64_t *)sm;
   int *ibuf = (int *)(sm + 2);

@@ -35,9 +35,10 @@ def make_settings(args: dict | None) -> _lib.BconeSettings:
         if k == "eps":  # diffcp maps eps -> eps_abs = eps_rel for SCS >= 3 (SURVEY.md 8a F7)
             st.eps_abs = float(v)
             st.eps_rel = float(v)
-        elif k == "mode":
-            if v not in ("lsqr",):
-                raise ValueError(f"backward mode {v!r} is not supported (only 'lsqr')")
+        elif k == "mode":   # diffcp's least-squares solver for the derivatives: LSQR or LSMR ("dense" is not built)
+            if v not in ("lsqr", "lsmr"):
+                raise ValueError(f"backward mode {v!r} is not supported (only 'lsqr' and 'lsmr')")
+            st.lsmr = 1 if v == "lsmr" else 0
         elif k in _ARG_MAP:
             cur = getattr(st, _ARG_MAP[k])
             setattr(st, _ARG_MAP[k], type(cur)(v))

@@ -54,6 +54,9 @@ typedef struct {
   int32_t acceleration_lookback;       /* SCS: Anderson acceleration window; 10 (type-I), < 0 type-II, 0 off
                                           (what the reference's tests pass, tests/test_torch.py:401-405); |.| <= 16 */
   int32_t acceleration_interval;       /* SCS: accelerate every this many iterations (10)                    */
+  int32_t lsmr;                        /* least-squares solver of bcone_vjp / bcone_jvp (diffcp's mode): 0 LSQR (default), 1 LSMR
+                                          (SciPy's lsmr, damp = 0).  LSMR uses lsqr_atol, lsqr_btol, lsqr_conlim, lsqr_iter_lim
+                                          and lsqr_precond as LSQR does */
 } bcone_settings;
 
 enum { BCONE_SOLVED = 1, BCONE_INACCURATE = 2, BCONE_UNBOUNDED = -1, BCONE_INFEASIBLE = -2, BCONE_FAILED = -4 };
