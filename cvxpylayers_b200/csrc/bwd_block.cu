@@ -11,8 +11,16 @@
 // W = L^{-1} A_L'  (overwrites the staged rows of A in place) and  S = W'W = A_L P^{-1} A_L'  (Cholesky +
 // inverse).  Only the live rows of A are staged (one TMA bulk copy per row).  Instances where the
 // factorisation does not apply (P not positive definite, A_L rank deficient, more live rows than
-// variables) are appended to a device-side list and re-run by bwd_fast_kernel with lsqr_precond = 1.
+// variables, or W and S together larger than the m n doubles the rows are staged in) are appended to a
+// device-side list and re-run by bwd_fast_kernel with lsqr_precond = 1.
 #include "common.cuh"
+
+// W (nl x n) and then S (nl x nl, packed lower) are written into the buffer of m n doubles that stages the live rows.  With nl
+// close to m and m < 1.5 n (e.g. every row an equality) S would run past it into the vectors and the factorisation scratch.
+// (Staging the rows themselves always fits: nl <= m.)
+__device__ __forceinline__ bool blk_fits(int nl, int n, int m) {
+  return nl <= n && nl * n + ((nl * (nl + 1)) >> 1) <= ((m * n + 1) & ~1);
+}
 
 struct BlkSmem {
   double *Pb, *Ab, *x, *c, *px2c, *piy, *hp, *q, *rhs, *z, *U, *V, *W, *tn, *t2, *tL, *ry, *part, *red;
@@ -114,7 +122,7 @@ __device__ __forceinline__ void bwd_block_body(const BwdArgs a) {   // (by value
     }
     __syncthreads();
     const int nl = M.ibuf[1], nr = n + nl;
-    bool applicable = nl <= n;
+    bool applicable = blk_fits(nl, n, m);
     if (applicable && !a.use_tma) {
       for (int e = t; e < nl * n; e += T) { const int l = e / n, j = e - l * n; M.Ab[e] = Ag[(size_t)M.live[l] * n + j]; }
     }

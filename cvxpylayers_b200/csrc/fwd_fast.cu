@@ -52,7 +52,7 @@ struct Geo {
   __host__ __device__ __forceinline__ int rowsR() const { return mpad() > npad() ? mpad() : npad(); }
   // X region during the iterations: [Kinv npad x kst | partial sums (column partials RTu x npad and row partials
   // rowsR x CT take turns) | private tile slots TR x FT double2]; it also stages A (m x n) for the K formation,
-  // and during the Ruiz passes (no Kinv yet) the row partials sit at its start.
+  // and during the Ruiz passes (no Kinv yet) it holds their row partials (oRz).
   // Row stride of Kinv.  The 2 x 10 tiles of kinv_rows are read as double2 by quarter-warps that straddle two tile rows
   // (10 tiles per row, 8 lanes per quarter); with 16-byte units u = KR R kst / 2 + 5 C + c / 2 the two halves collide unless
   // KR kst / 2 = 2 (mod 8): stride 100 costs 60 % extra wavefronts on the 80 KB that every iteration reads, 106 none.
@@ -63,6 +63,10 @@ struct Geo {
   __host__ __device__ __forceinline__ int szPart() const { const int a = RTu() * npad(), b = rowsR() * CT(); return ((a > b ? a : b) + 1) & ~1; }
   __host__ __device__ __forceinline__ int oPS() const { return oXC() + szPart(); }
   __host__ __device__ __forceinline__ int XD() const { const int it = oPS() + TR * FT * (TC - TCR), stg = mpad() * npad(); return ((it > stg ? it : stg) + 1) & ~1; }
+  // Row partials of the Ruiz passes (rowsR x CT), written in the same phase as the column partials at oXC: in the Kinv area,
+  // unused then, unless they would reach oXC (m >> n); then behind the private tile slots, where A was staged (ok() checks
+  // that they end inside X; XD itself is left alone: its formula feeds every vector offset of the iteration loop).
+  __host__ __device__ __forceinline__ int oRz() const { return rowsR() * CT() <= oXC() ? 0 : oPS() + TR * FT * (TC - TCR); }
   // whole block (doubles): [bar, ibuf (4) | X | Li | 9 x-vectors | 7 y-vectors | red (8 x 32) | scalars (64) | Cholesky scratch]
   __host__ __device__ __forceinline__ int oX() const { return 4; }
   __host__ __device__ __forceinline__ int oLi() const { return oX() + XD(); }
@@ -81,7 +85,8 @@ struct Geo {
   __host__ __device__ __forceinline__ int cK() const { return cD() + mpad(); }
   __host__ __device__ __forceinline__ int cTotal() const { return (cK() + npad() * kst() + 1) & ~1; }
   __host__ __device__ __forceinline__ bool ok(int n, int m) const {
-    return n <= FT && m <= FT && CT() * RTu() <= FT && ((npad() + KR() - 1) / KR()) * CT() <= FT && chol_scratch_doubles(npad(), FT) <= szCh();
+    return n <= FT && m <= FT && CT() * RTu() <= FT && ((npad() + KR() - 1) / KR()) * CT() <= FT && chol_scratch_doubles(npad(), FT) <= szCh() &&
+           oRz() + rowsR() * CT() <= XD();
   }
 };
 
@@ -670,7 +675,7 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
       for (int r = 0; r < TR; r++) ps[r * FT] = sl[r];
     };
     load_tile();
-    double *const XRz = X;   // row partials of the Ruiz passes (the Kinv area is still unused)
+    double *const XRz = X + g.oRz();   // row partials of the Ruiz passes
     pt_stamp(0);
 
     // ---- Ruiz equilibration: A^ = D A E, P^ = E P E (SURVEY.md 8a F4) ----

@@ -24,10 +24,15 @@ def _same(a, b):
     return all(torch.equal(getattr(a, k), getattr(b, k)) for k in ("x", "y", "s", "status", "iters"))
 
 
-@pytest.mark.parametrize("shape", [(100, 200, 50), (80, 200, 40), (75, 190, 30)])   # the compile-time geometry and two runtime ones
+# the compile-time geometry and two runtime ones at B = 96; then, at B = 16 (the oracle checks below run on the CPU), shape
+# classes of tests/tiled_shapes.py: 4-row K^-1 tiles at the shared-memory limit, n > m, the compile-time geometry at its widest
+# padding with odd m n.  (The classes with m >> n are not here: dense_qp plants more active rows than variables there, and the
+# perturbed b below then has no feasible point; tests/test_gpu_tiled_shapes.py runs them on planted batches.)
+@pytest.mark.parametrize("shape", [(100, 200, 50, 96), (80, 200, 40, 96), (75, 190, 30, 96),
+                                   (110, 136, 30, 16), (101, 93, 10, 16), (91, 197, 20, 16)])
 def test_cached_setup_is_the_uncached_algorithm(cuda_device, shape):
-    n, m, z = shape
-    B, dev = 96, cuda_device
+    n, m, z, B = shape
+    dev = cuda_device
     bt = pr.dense_qp(B, n, m, z, seed=21)
     st = bt.structure
     eng = Engine(st, dev)

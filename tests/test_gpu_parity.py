@@ -170,12 +170,18 @@ def _two_engines(st, dev, monkeypatch):
     return fast, generic
 
 
-@pytest.mark.parametrize("shape", [(100, 200, 50, True), (80, 200, 30, True), (75, 190, 20, True), (90, 170, 0, False)])
+@pytest.mark.parametrize("shape", [(100, 200, 50, True), (80, 200, 30, True), (75, 190, 20, True), (90, 170, 0, False),
+                                   # the shape classes of tests/tiled_shapes.py
+                                   (110, 136, 30, True), (101, 93, 10, True), (102, 100, 20, True), (110, 93, 93, True),
+                                   (11, 509, 0, True), (40, 512, 10, True), (91, 197, 20, True), (99, 199, 50, True),
+                                   (57, 333, 0, True), (66, 160, 16, True)])
 @pytest.mark.parametrize("eps", [1e-4, 1e-9])
 def test_tiled_forward_equals_generic_forward(shape, eps, cuda_device, monkeypatch):
     """The register-tiled kernel is the same algorithm as fwd.cu: identical iteration counts and solutions that
     differ only by summation order, on the compile-time geometry (100 x 200), on runtime geometries with column /
-    row padding (80 x 200, 75 x 190) and on an LP without a quadratic term; both against the oracle's certificate."""
+    row padding (80 x 200, 75 x 190) and on an LP without a quadratic term; both against the oracle's certificate.
+    Then on a representative of every shape class of tests/tiled_shapes.py: 4-row K^-1 tiles, n > m, every row an equality,
+    half and all of the CTA holding tiles, odd m n (plain-load staging), the compile-time geometry at its widest padding."""
     n, m, z, with_P = shape
     bt = pr.dense_qp(B=12, n=n, m=m, z=z, seed=11, with_P=with_P)
     st, dev = bt.structure, cuda_device
@@ -187,11 +193,11 @@ def test_tiled_forward_equals_generic_forward(shape, eps, cuda_device, monkeypat
     A, b, c, P = _t(bt.A_vals, dev), _t(bt.b, dev), _t(bt.c, dev), _t(bt.P_vals, dev)
     s1, s2 = fast.solve(A, b, c, P, args), generic.solve(A, b, c, P, args)
     torch.cuda.synchronize()
-    assert (s1.status == s2.status).all(), (s1.status, s2.status)
+    assert (s1.status == s2.status).all(), (shape, s1.status, s2.status)
     # same checks at the same iterations; at the tight tolerance a residual that sits within rounding of its
     # threshold may cross it one check later in one of the two summation orders
     di = (s1.iters - s2.iters).abs()
-    assert int(di.max()) <= (0 if eps > 1e-6 else 25) and int((di > 0).sum()) <= bt.B // 4, (s1.iters, s2.iters)
+    assert int(di.max()) <= (0 if eps > 1e-6 else 25) and int((di > 0).sum()) <= bt.B // 4, (shape, s1.iters, s2.iters)
     solved = (s1.status.cpu().numpy() == 1)
     assert solved.all() or not with_P   # (plain operator splitting may need more than 50000 iterations on an LP)
     scale = max(1.0, float(s2.x.abs().max()))
