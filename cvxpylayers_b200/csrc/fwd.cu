@@ -466,9 +466,15 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) fwd_kernel(c
       // Warm start (SURVEY.md 8f.2; the reference exposes it for one backend only, torch/cvxpylayer.py:464-487): start the
       // splitting at the fixed point a previous solution (x0, y0, s0) would be for this instance -- w = u + R^{-1} v with
       // u = (x0 sigma / E, y0 sigma / D, 1), v_y = s0 D sigma (the inverse of the write-back below at tau = 1).
+      // A row with a non-finite value (the NaN rows of a non-solved instance) starts cold: from it tau never turns positive.
       const double *x0 = a.x0 + (size_t)inst * n, *y0 = a.y0 + (size_t)inst * m, *s0 = a.s0 + (size_t)inst * m;
-      for (int j = t; j < n; j += T) M.w[j] = x0[j] * sigma / M.En[j];
-      for (int i = t; i < m; i += T) M.w[n + i] = y0[i] * sigma / M.Dm[i] + s0[i] * M.Dm[i] * sigma * inv_ry(S, i, scale);
+      bool bad = false;
+      for (int j = t; j < n; j += T) bad |= !isfinite(x0[j]);
+      for (int i = t; i < m; i += T) bad |= !isfinite(y0[i]) || !isfinite(s0[i]);
+      if (!__syncthreads_or(bad)) {
+        for (int j = t; j < n; j += T) M.w[j] = x0[j] * sigma / M.En[j];
+        for (int i = t; i < m; i += T) M.w[n + i] = y0[i] * sigma / M.Dm[i] + s0[i] * M.Dm[i] * sigma * inv_ry(S, i, scale);
+      }
     }
     if (INDIRECT) for (int j = t; j < n; j += T) M.cx[j] = 0.0;
     __syncthreads();

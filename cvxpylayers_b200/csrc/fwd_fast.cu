@@ -777,10 +777,14 @@ __global__ void __launch_bounds__(FT, 1) fwd_fast_kernel(const __grid_constant__
     int it = 0, next_check = st.adaptive_check ? (st.check_interval < 10 ? st.check_interval : 10) : st.check_interval;
     if (t < n) { vx(VX_W)[t] = 0; vx(VX_U)[t] = 0; vx(VX_UT)[t] = 0; }
     if (t < m) { vy(VY_W)[t] = 0; vy(VY_U)[t] = 0; vy(VY_UT)[t] = 0; }
-    if (a.x0) {   // warm start: w = u + R^{-1} v at the previous solution (see fwd.cu)
+    if (a.x0) {   // warm start: w = u + R^{-1} v at the previous solution; a row with a non-finite value starts cold (see fwd.cu)
       const double sg = sc[SC_SIGMA];
-      if (t < n) vx(VX_W)[t] = a.x0[(size_t)inst * n + t] * sg / vx(VX_EN)[t];
-      if (t < m) { const double d = vy(VY_DM)[t]; vy(VY_W)[t] = a.y0[(size_t)inst * m + t] * sg / d + a.s0[(size_t)inst * m + t] * d * sg * inv_ry_f(z, t, scale); }
+      const double x0 = t < n ? a.x0[(size_t)inst * n + t] : 0.0, y0 = t < m ? a.y0[(size_t)inst * m + t] : 0.0,
+                   s0 = t < m ? a.s0[(size_t)inst * m + t] : 0.0;
+      if (!__syncthreads_or(!isfinite(x0) || !isfinite(y0) || !isfinite(s0))) {
+        if (t < n) vx(VX_W)[t] = x0 * sg / vx(VX_EN)[t];
+        if (t < m) { const double d = vy(VY_DM)[t]; vy(VY_W)[t] = y0 * sg / d + s0 * d * sg * inv_ry_f(z, t, scale); }
+      }
     }
     __syncthreads();
     bool refactor = true, first = true;

@@ -674,7 +674,11 @@ static int solve_impl(const orc_desc *d, const double *Av, const double *Pv, con
   double rp = NAN, rd = NAN, gap = NAN;
   if (factor(&W)) { status = ORC_FAILED; goto done; }
   w[N - 1] = 1.0;
-  if (x0 && y0 && s0) {
+  /* a warm start with a non-finite value (the NaN outputs of a non-solved instance) starts cold: from it tau never turns positive */
+  int warm_ok = x0 && y0 && s0;
+  for (int j = 0; warm_ok && j < n; j++) warm_ok = isfinite(x0[j]);
+  for (int i = 0; warm_ok && i < m; i++) warm_ok = isfinite(y0[i]) && isfinite(s0[i]);
+  if (warm_ok) {
     for (int j = 0; j < n; j++) w[j] = x0[j] * sigma / W.E[j];
     for (int i = 0; i < m; i++) w[n + i] = y0[i] * sigma / W.D[i] + s0[i] * W.D[i] * sigma / W.ry[i];
   }
