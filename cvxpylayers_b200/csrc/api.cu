@@ -51,6 +51,16 @@ const Plan &pick(const TieredPlan &t, int B, int num_sms, int small_mode) {
 // CTAs of the largest grid either build launches: what the per-CTA slabs are sized for
 size_t max_grid(const TieredPlan &t, int num_sms) { return (size_t)num_sms * std::max(t.big.ctas, t.has_small ? t.small.ctas : 0); }
 
+// The backward plans of one least-squares method (settings.lsmr: [0] LSQR, [1] LSMR), each with a flag saying it exists.
+// gen / jvp: the generic kernel (bwd.cu) as the adjoint and as the forward mode; fast: the fused single-pass adjoint (bwd_fast.cu;
+// dense A, polyhedral cones, dense-or-no P), which runs instead of gen where it exists; block: the KKT-block preconditioned
+// adjoint (bwd_block.cu, lsqr_precond = 2), whose rejected instances take a second pass on fast, else gen.
+struct LsPlans {
+  TieredPlan gen, jvp;
+  Plan fast, block;
+  bool gen_ok = false, jvp_ok = false, fast_ok = false, block_ok = false;
+};
+
 struct Handle {
   DevStruct S{};
   int device = 0, max_batch = 0, num_sms = 0;
@@ -66,29 +76,20 @@ struct Handle {
   PMap pmA, pmq, pmP;
   int P1 = 0;
   int tma_ok = 0, psd_total = 0;
-  // Launch plans, chosen once in bcone_create.  The generic kernels (fwd.cu; bwd.cu as adjoint and as forward mode) each have a
-  // TieredPlan; fast_fwd / fast_bwd / block_bwd say where a specialised kernel runs instead.
-  TieredPlan fwd, bwd;
-  // forward-mode derivative (bcone_jvp): always the generic kernel (bwd.cu, JVP = true), so structures on the fused backward
-  // need a generic geometry of their own; chosen by the same rule as the generic backward's.  jvp_ok = 0: none fits.
-  TieredPlan jvp; int jvp_ok = 0;
+  // Launch plans, chosen once in bcone_create.  The generic forward (fwd.cu) has a TieredPlan; fast_fwd says where the
+  // register-tiled forward runs instead.  The backward plans are per least-squares method.
+  TieredPlan fwd;
   Plan fwd_fast;    // fast_fwd: dense A, polyhedral cones, direct mode: register-tiled forward (fwd_fast.cu)
-  Plan bwd_fast;    // fast_bwd: dense A, polyhedral cones, dense-or-no P: fused single-pass backward (bwd_fast.cu)
-  Plan bwd_block;   // block_bwd: KKT-block preconditioned backward (lsqr_precond = 2)
-  int fast_fwd = 0, fast_bwd = 0, block_bwd = 0;
-  // LSMR (settings.lsmr = 1): the same plans for the LSMR kernels, which keep one more N-vector, chosen by the same rules.  A
-  // structure on the fused backward whose fused geometry has no room for that vector runs the generic LSMR kernel
-  // (bwd_lsmr); the block-preconditioned LSMR hands the instances it rejects to whichever of the two runs.
-  TieredPlan bwd_lsmr, jvp_lsmr; int bwd_lsmr_ok = 0, jvp_lsmr_ok = 0;
-  Plan bwd_fast_lsmr, bwd_block_lsmr;
-  int fast_bwd_lsmr = 0, block_bwd_lsmr = 0;
+  int fast_fwd = 0;
+  LsPlans ls[2];
   int small_mode = 1;   // BCONE_SMALL_CTA: 0 disables the 4-CTA/SM builds, 2 forces them
   // Per-stream scratch slabs (one per CTA of the grid): launches on different streams may overlap, launches on one
   // stream cannot, so the stream is the unit of ownership.  Allocated on first use.
   // shared matrices: setup = the batch's one set-up record of the register-tiled forward (+ the outputs of its set-up launch),
   // srec / part = the adjoint's per-instance r, pi_y records and the reduction's partial sums (shared.cu)
-  struct StreamWs { cudaStream_t s; double *fwd = nullptr, *bwd = nullptr, *aa = nullptr, *park = nullptr, *jvp = nullptr; size_t aa_cap = 0;
-                    double *bwd_lsmr = nullptr, *jvp_lsmr = nullptr;
+  // bwd / jvp: the generic backward's vector slabs, per least-squares method
+  struct StreamWs { cudaStream_t s; double *fwd = nullptr, *aa = nullptr, *park = nullptr; size_t aa_cap = 0;
+                    double *bwd[2] = {nullptr, nullptr}, *jvp[2] = {nullptr, nullptr};
                     double *setup = nullptr, *srec = nullptr, *part = nullptr; size_t srec_cap = 0, part_cap = 0; };
   std::vector<StreamWs> sws;
   int *fail_list[RING] = {nullptr}; int fail_cap[RING] = {0};
@@ -328,43 +329,39 @@ int plan_lsqr(Handle *h, const Limits &L, TieredPlan &t, int jvp, int lsmr) {
   return BCONE_OK;
 }
 
-// Fused single-pass backward (bwd_fast.cu) and, on top of it, the block-preconditioned variant for strongly convex QPs, where
-// the structure allows them.  Sets fast_bwd / block_bwd; BCONE_ECUDA (message set) if the fused kernel cannot be configured.
-int plan_fast(Handle *h, const Limits &L) {
+// The backward plans of one least-squares method (lsmr: LSMR, whose kernels keep one more N-vector), planned after LSQR's.
+// The fused adjoint where the structure allows it and it fits (needing N more doubles at the same thread count, LSMR's exists
+// only where LSQR's does); the block-preconditioned adjoint on top of LSQR's fused one, for strongly convex QPs (LSMR's where
+// LSQR's configured: its shared memory does not depend on the method); the generic adjoint where there is no fused one; the
+// generic forward mode always.  Returns the adjoint's BCONE_OK, BCONE_EUNSUPPORTED (no tier fits) or BCONE_ECUDA (message set);
+// only LSQR's adjoint is required (bcone_create fails without it), so for LSMR a missing fused plan falls back to the generic
+// one, and a missing adjoint disables the block pass (there is no pass for the instances it rejects).
+int plan_backward(Handle *h, const Limits &L, int lsmr) {
   const DevStruct &S = h->S;
   const int n = S.n, m = S.m;
-  if (!(S.dense && S.ncones == 0 && S.ep + S.ed == 0 && n <= 128 && (n % 2) == 0 && (S.nnzP == 0 || S.p_dense))) return BCONE_OK;
-  for (int tt = L.threads; tt >= 64; tt /= 2) {
-    size_t sm = bc_bwdf_smem_bytes(n, m, S.nnzA, S.nnzP, tt, 0);
-    if (sm <= L.smem_cap) { h->fast_bwd = 1; h->bwd_fast = Plan{bc_bwdf_kernel(n, 0), tt, sm}; break; }
-  }
-  if (!h->fast_bwd) return BCONE_OK;
-  const cudaError_t e = configure(h->bwd_fast);
-  if (e != cudaSuccess) return cuda_fail(nullptr, e, "cudaFuncSetAttribute");
-  if (S.nnzP > 0 && 6 * (n + m + 1) >= 8 * n + 72)
-    for (int tt = L.threads; tt >= 128; tt /= 2) {
-      size_t sm = bc_bwdb_smem_bytes(n, m, tt);
-      if (sm <= L.smem_cap) { h->bwd_block = Plan{bc_bwdb_kernel(0), tt, sm}; h->block_bwd = configure(h->bwd_block) == cudaSuccess; break; }
+  LsPlans &p = h->ls[lsmr];
+  if (S.dense && S.ncones == 0 && S.ep + S.ed == 0 && n <= 128 && (n % 2) == 0 && (S.nnzP == 0 || S.p_dense))
+    for (int tt = L.threads; tt >= 64; tt /= 2) {
+      const size_t sm = bc_bwdf_smem_bytes(n, m, S.nnzA, S.nnzP, tt, lsmr);
+      if (sm <= L.smem_cap) {
+        p.fast = Plan{bc_bwdf_kernel(n, lsmr), tt, sm};
+        const cudaError_t e = configure(p.fast);
+        if (e != cudaSuccess && !lsmr) return cuda_fail(nullptr, e, "cudaFuncSetAttribute");
+        p.fast_ok = e == cudaSuccess;
+        break;
+      }
     }
-  return BCONE_OK;
-}
-
-// The LSMR variants of the fused and the block-preconditioned backward, where the LSQR ones run.  The fused one keeps one more
-// N-vector, searched for by the same rule; where it does not fit (C2: A and P fill shared memory), the generic LSMR kernel runs
-// the adjoint.  The block-preconditioned one needs no more shared memory than its LSQR twin and takes its geometry; the
-// instances it rejects go to the fused LSMR kernel, or to the generic one (bcone_create checks that one of them exists).
-void plan_fast_lsmr(Handle *h, const Limits &L) {
-  const DevStruct &S = h->S;
-  const int n = S.n, m = S.m;
-  if (!h->fast_bwd) return;
-  for (int tt = L.threads; tt >= 64; tt /= 2) {
-    const size_t sm = bc_bwdf_smem_bytes(n, m, S.nnzA, S.nnzP, tt, 1);
-    if (sm <= L.smem_cap) { h->bwd_fast_lsmr = Plan{bc_bwdf_kernel(n, 1), tt, sm}; h->fast_bwd_lsmr = configure(h->bwd_fast_lsmr) == cudaSuccess; break; }
-  }
-  if (h->block_bwd) {
-    h->bwd_block_lsmr = h->bwd_block; h->bwd_block_lsmr.fn = bc_bwdb_kernel(1);
-    h->block_bwd_lsmr = configure(h->bwd_block_lsmr) == cudaSuccess;
-  }
+  if (h->ls[0].fast_ok && (!lsmr || h->ls[0].block_ok) && S.nnzP > 0 && 6 * (n + m + 1) >= 8 * n + 72)
+    for (int tt = L.threads; tt >= 128; tt /= 2) {
+      const size_t sm = bc_bwdb_smem_bytes(n, m, tt);
+      if (sm <= L.smem_cap) { p.block = Plan{bc_bwdb_kernel(lsmr), tt, sm}; p.block_ok = configure(p.block) == cudaSuccess; break; }
+    }
+  const int rc = p.fast_ok ? BCONE_OK : plan_lsqr(h, L, p.gen, 0, lsmr);
+  if (rc != BCONE_OK && !lsmr) return rc;
+  p.gen_ok = !p.fast_ok && rc == BCONE_OK;
+  if (rc != BCONE_OK) p.block_ok = false;
+  p.jvp_ok = plan_lsqr(h, L, p.jvp, 1, lsmr) == BCONE_OK;
+  return rc;
 }
 
 // With values and vectors off chip, what is left in shared memory is the per-CTA scratch: the cone scratch (per-warp PSD
@@ -416,21 +413,15 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
   const Limits L = limits(h, prop.sharedMemPerBlockOptin);
   const char *sc = getenv("BCONE_SMALL_CTA");
   h->small_mode = sc ? atoi(sc) : 1;
-  const int rfast = plan_fast(h, L);
   int rc = plan_forward(h, L);
-  const int rb = h->fast_bwd ? rfast : plan_lsqr(h, L, h->bwd, 0, 0);
+  const int rb = plan_backward(h, L, 0);
   if (rc == BCONE_OK || rb == BCONE_EUNSUPPORTED) rc = rb;   // "does not fit" comes before a CUDA error
   if (rc == BCONE_EUNSUPPORTED) return give_up(rc, explain_no_fit(h, d, L.smem_cap));
   if (rc != BCONE_OK) return give_up(rc, g_create_err);
   h->tma_ok = (d->nnzA > 0 && (d->nnzA % 2) == 0 && (size_t)d->nnzA * 8 < (1u << 20)) ? 1 : 0;
-  // forward-mode derivative: the generic geometry (the backward's own when the backward is generic).  A structure without
-  // one is still accepted; only bcone_jvp refuses it.
-  h->jvp_ok = plan_lsqr(h, L, h->jvp, 1, 0) == BCONE_OK;
-  // LSMR (settings.lsmr = 1): likewise; a structure without an LSMR geometry is accepted, only LSMR calls refuse it
-  plan_fast_lsmr(h, L);
-  h->bwd_lsmr_ok = h->fast_bwd_lsmr || plan_lsqr(h, L, h->bwd_lsmr, 0, 1) == BCONE_OK;
-  if (!h->bwd_lsmr_ok) h->block_bwd_lsmr = 0;   // (no pass for the instances it rejects)
-  h->jvp_lsmr_ok = plan_lsqr(h, L, h->jvp_lsmr, 1, 1) == BCONE_OK;
+  // A structure without an LSMR adjoint or without a forward-mode geometry (either method) is still accepted; only the calls
+  // that need them refuse it.
+  plan_backward(h, L, 1);
   cudaGetLastError();   // (a refused configuration is not an error of this call)
   *out = h;
   return BCONE_OK;
@@ -788,12 +779,10 @@ static int vjp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !dx || !dy || !dA_vals || !db || !dc || !stg)
     return fail(h, BCONE_EINVAL, "vjp: null argument");
   if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "vjp: structure has P but P_vals is NULL");
-  // the LSQR or the LSMR kernels (settings.lsmr)
-  const bool lsmr = stg->lsmr != 0;
-  if (lsmr && !h->bwd_lsmr_ok) return fail(h, BCONE_EUNSUPPORTED, "vjp: the instance does not fit the LSMR kernels");
-  const TieredPlan &gen = lsmr ? h->bwd_lsmr : h->bwd;
-  const int fast_bwd = lsmr ? h->fast_bwd_lsmr : h->fast_bwd, block_bwd = lsmr ? h->block_bwd_lsmr : h->block_bwd;
-  const Plan &bwd_fast = lsmr ? h->bwd_fast_lsmr : h->bwd_fast, &bwd_block = lsmr ? h->bwd_block_lsmr : h->bwd_block;
+  const int lsmr = stg->lsmr != 0;   // the LSQR or the LSMR kernels
+  const LsPlans &p = h->ls[lsmr];
+  if (!p.fast_ok && !p.gen_ok) return fail(h, BCONE_EUNSUPPORTED, "vjp: the instance does not fit the LSMR kernels");   // (LSQR's exist)
+  const TieredPlan &gen = p.gen;
   cudaStream_t st = (cudaStream_t)stream;
   BwdArgs a;
   a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
@@ -823,34 +812,33 @@ static int vjp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   CK(cudaSetDevice(h->device), "vjp set device");
   a.ws = nullptr; a.ws_stride = (long long)gen.ws_stride;
   if (gen.vec_global) {
-    double **slab = lsmr ? &sw->bwd_lsmr : &sw->bwd;
-    if (!ensure_slab(h, slab, nullptr, gen.ws_stride * max_grid(gen, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc backward workspace");
-    a.ws = *slab;
+    if (!ensure_slab(h, &sw->bwd[lsmr], nullptr, gen.ws_stride * max_grid(gen, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc backward workspace");
+    a.ws = sw->bwd[lsmr];
   }
   a.inst_list = nullptr; a.B_dev = nullptr; a.fail_list = nullptr; a.fail_count = nullptr; a.prof = h->prof;
-  if (block_bwd && stg->lsqr_precond == 2) {
+  if (p.block_ok && stg->lsqr_precond == 2) {
     // pass 1: block-preconditioned solve; pass 2: equilibrated LSQR on the instances it rejected
     if (h->fail_cap[slot] < B) {
-      int *p = nullptr;
-      CK(cudaMalloc((void **)&p, (size_t)B * sizeof(int)), "vjp fail list");
-      h->allocs.push_back(p); h->fail_list[slot] = p; h->fail_cap[slot] = B;
+      int *q = nullptr;
+      CK(cudaMalloc((void **)&q, (size_t)B * sizeof(int)), "vjp fail list");
+      h->allocs.push_back(q); h->fail_list[slot] = q; h->fail_cap[slot] = B;
     }
     CK(cudaMemsetAsync(ctr + 1, 0, 3 * sizeof(int), st), "vjp counters");
     h->last_block_slot = slot;
     a.fail_list = h->fail_list[slot]; a.fail_count = ctr + 2;
-    CK(launch(bwd_block, std::min(B, h->num_sms), &a, st), "vjp launch (block)");
+    CK(launch(p.block, std::min(B, h->num_sms), &a, st), "vjp launch (block)");
     BwdArgs f = a;
     f.st.lsqr_precond = 1; f.counter = ctr + 3; f.inst_list = h->fail_list[slot]; f.B_dev = ctr + 2;
     f.fail_list = nullptr; f.fail_count = nullptr;
-    const Plan &second = fast_bwd ? bwd_fast : pick(gen, B, h->num_sms, h->small_mode);   // (LSQR: always the fused kernel)
+    const Plan &second = p.fast_ok ? p.fast : pick(gen, B, h->num_sms, h->small_mode);   // (LSQR: always the fused kernel)
     CK(launch(second, grid_for(second, B, h->num_sms), &f, st), "vjp launch (fallback)");
     h->launches += 2;
     return reduce();
   }
   if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // block factorisation not available for this structure
   CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "vjp counter");
-  const Plan &plan = fast_bwd ? bwd_fast : pick(gen, B, h->num_sms, h->small_mode);
-  CK(launch(plan, grid_for(plan, B, h->num_sms), &a, st), fast_bwd ? "vjp launch (fast)" : "vjp launch");
+  const Plan &plan = p.fast_ok ? p.fast : pick(gen, B, h->num_sms, h->small_mode);
+  CK(launch(plan, grid_for(plan, B, h->num_sms), &a, st), p.fast_ok ? "vjp launch (fast)" : "vjp launch");
   h->launches++;
   return reduce();
 }
@@ -875,10 +863,10 @@ static int jvp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !dA_vals || !db || !dc || !dx || !dy || !stg)
     return fail(h, BCONE_EINVAL, "jvp: null argument");
   if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "jvp: structure has P but P_vals is NULL");
-  const bool lsmr = stg && stg->lsmr != 0;   // the LSQR or the LSMR kernel (settings.lsmr)
-  if (!lsmr && !h->jvp_ok) return fail(h, BCONE_EUNSUPPORTED, "jvp: the instance does not fit the generic LSQR kernel");
-  if (lsmr && !h->jvp_lsmr_ok) return fail(h, BCONE_EUNSUPPORTED, "jvp: the instance does not fit the generic LSMR kernel");
-  const TieredPlan &gen = lsmr ? h->jvp_lsmr : h->jvp;
+  const int lsmr = stg->lsmr != 0;   // the LSQR or the LSMR kernel
+  if (!h->ls[lsmr].jvp_ok)
+    return fail(h, BCONE_EUNSUPPORTED, lsmr ? "jvp: the instance does not fit the generic LSMR kernel" : "jvp: the instance does not fit the generic LSQR kernel");
+  const TieredPlan &gen = h->ls[lsmr].jvp;
   cudaStream_t st = (cudaStream_t)stream;
   BwdArgs a{};
   a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
@@ -893,9 +881,8 @@ static int jvp_impl(Handle *h, int32_t B, const double *A_vals, const double *P_
   a.ws_stride = (long long)gen.ws_stride;
   if (gen.vec_global) {
     Handle::StreamWs *sw = stream_ws(h, st);
-    double **slab = lsmr ? &sw->jvp_lsmr : &sw->jvp;
-    if (!ensure_slab(h, slab, nullptr, gen.ws_stride * max_grid(gen, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc jvp workspace");
-    a.ws = *slab;
+    if (!ensure_slab(h, &sw->jvp[lsmr], nullptr, gen.ws_stride * max_grid(gen, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc jvp workspace");
+    a.ws = sw->jvp[lsmr];
   }
   a.prof = h->prof;
   CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "jvp counter");
@@ -965,7 +952,8 @@ extern "C" int bcone_path_info(void *handle, int32_t *fwd_path, int32_t *bwd_pat
     else if (h->fwd.vals_global) *fwd_path = h->fwd.indirect ? 6 : (h->fwd.factor_global ? 5 : 4);
     else *fwd_path = h->fwd.indirect ? 1 : (h->fwd.factor_global ? 3 : 0);
   }
-  if (bwd_path) *bwd_path = h->block_bwd ? 2 : (h->fast_bwd ? 1 : (h->bwd.vals_global ? 3 : 0));
+  const LsPlans &p = h->ls[0];   // (the LSQR plans)
+  if (bwd_path) *bwd_path = p.block_ok ? 2 : (p.fast_ok ? 1 : (p.gen.vals_global ? 3 : 0));
   return BCONE_OK;
 }
 
@@ -973,14 +961,15 @@ extern "C" int bcone_small_cta_info(void *handle, int32_t *fwd_small_ctas, int32
   Handle *h = (Handle *)handle;
   if (!h) return BCONE_EINVAL;
   if (fwd_small_ctas) *fwd_small_ctas = h->fwd.has_small ? h->fwd.small.ctas : 0;
-  if (bwd_small_ctas) *bwd_small_ctas = h->bwd.has_small ? h->bwd.small.ctas : 0;
+  if (bwd_small_ctas) *bwd_small_ctas = h->ls[0].gen.has_small ? h->ls[0].gen.small.ctas : 0;   // (the LSQR plans)
   return BCONE_OK;
 }
 
 extern "C" int bcone_kernel_info(void *handle, int32_t *ft, int32_t *fs, int32_t *fc, int32_t *bt, int32_t *bs, int32_t *bcx) {
   Handle *h = (Handle *)handle;
   if (!h) return BCONE_EINVAL;
-  const Plan &f = h->fast_fwd ? h->fwd_fast : h->fwd.big, &b = h->fast_bwd ? h->bwd_fast : h->bwd.big;
+  const LsPlans &p = h->ls[0];   // (the LSQR plans)
+  const Plan &f = h->fast_fwd ? h->fwd_fast : h->fwd.big, &b = p.fast_ok ? p.fast : p.gen.big;
   if (ft) *ft = f.threads; if (fs) *fs = (int32_t)f.smem; if (fc) *fc = f.ctas;
   if (bt) *bt = b.threads; if (bs) *bs = (int32_t)b.smem; if (bcx) *bcx = b.ctas;
   return BCONE_OK;

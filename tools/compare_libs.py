@@ -4,9 +4,10 @@
 
 For every `problems.CONFIGS` entry and every BCONE_SMALL_CTA mode, each library (loaded through BCONE_LIB in a process of its
 own, because the mode is read when the handle is created) prints kernel_info(), path_info() and the launch_count() delta of one
-solve, one vjp and one jvp, at a batch below and at a batch above what the grid keeps resident (SMs x CTAs per SM).  The
-lines of the two libraries must be equal.  The vjp and the jvp run at a fixed point (the planted optimum, or library A's solution
-where the workload has none) and are deterministic, so their outputs must be bit-identical; the forward forms K with floating-point atomics on some paths (fwd.cu, factor_and_g),
+solve and of one vjp and one jvp for every lsqr_precond (0, 1, 2) and least-squares method (LSQR, LSMR), with the fallback_count()
+of the block-preconditioned vjp (lsqr_precond = 2), at a batch below and at a batch above what the grid keeps resident (SMs x CTAs
+per SM).  The lines of the two libraries must be equal.  The vjp and the jvp run at a fixed point (the planted optimum, or library
+A's solution where the workload has none) and are deterministic, so their outputs must be bit-identical; the forward forms K with floating-point atomics on some paths (fwd.cu, factor_and_g),
 so its solutions are compared at 1e-8 relative, the tolerance tests/test_gpu_large.py uses for the same reason.
 
 --timing instead prints, per library and alternating between them (order swapped every round), the host-clock time per call of
@@ -27,7 +28,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 FWD = {"eps": 1e-4, "max_iters": 100000}
-BWD = {"lsqr_precond": 1}
+BWD = [{"lsqr_precond": pc, "mode": mode} for pc in (0, 1, 2) for mode in ("lsqr", "lsmr")]
 
 
 def _setup(name, B, dev):
@@ -50,7 +51,7 @@ def worker(configs, outdir, at):
 
     dev = torch.device("cuda", 0)
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
-    fs, bs = make_settings(FWD), make_settings(BWD)
+    fs = make_settings(FWD)
     for name in configs:
         st, _ = _setup(name, 1, dev)
         info = Engine(st, dev).kernel_info()
@@ -67,19 +68,28 @@ def worker(configs, outdir, at):
             pt = [d["x_star"], d["y_star"], d["s_star"]]
             if pt[0] is None:
                 pt = torch.load(os.path.join(at, f"{name}_{B}.pt"))["solve"] if at else [sol.x, sol.y, sol.s]
-            vjp = eng.vjp(d["A_vals"], d["b"], d["c"], *pt, dx, dy, d["P_vals"], bs)
-            counts.append(eng.launch_count() - l0 - sum(counts))
-            try:
-                jvp = eng.jvp(d["A_vals"], d["b"], d["c"], *pt, tA, tb, tc, d["P_vals"], tP, bs)
-                counts.append(eng.launch_count() - l0 - sum(counts))
-            except RuntimeError as ex:   # a structure without a generic geometry: both libraries must refuse it alike
-                jvp = ()
-                counts.append(str(ex))
+            exact, fallbacks = [], []
+            for args in BWD:
+                bs = make_settings(args)
+                # (a structure without a geometry for the call -- the forward mode, or LSMR's adjoint: both libraries must refuse it alike)
+                for call in ("vjp", "jvp"):
+                    l1 = eng.launch_count()
+                    try:
+                        out = (eng.vjp(d["A_vals"], d["b"], d["c"], *pt, dx, dy, d["P_vals"], bs) if call == "vjp" else
+                               eng.jvp(d["A_vals"], d["b"], d["c"], *pt, tA, tb, tc, d["P_vals"], tP, bs))
+                        counts.append(eng.launch_count() - l1)
+                    except RuntimeError as ex:
+                        out = ()
+                        counts.append(str(ex))
+                    if call == "vjp" and args["lsqr_precond"] == 2:
+                        fallbacks.append(eng.fallback_count())
+                    exact += [v for v in out if v is not None]
             torch.cuda.synchronize()
-            torch.save({"solve": [sol.x, sol.y, sol.s], "status": [sol.status, sol.iters],
-                        "exact": [v for v in (*vjp, *jvp) if v is not None]}, os.path.join(outdir, f"{name}_{B}.pt"))
+            torch.save({"solve": [sol.x, sol.y, sol.s], "status": [sol.status, sol.iters], "exact": exact},
+                       os.path.join(outdir, f"{name}_{B}.pt"))
             print(json.dumps({"config": name, "B": B, "kernel_info": eng.kernel_info(), "path_info": eng.path_info(),
-                              "launches_solve_vjp_jvp": counts, "solved": int((sol.status == 1).sum())}), flush=True)
+                              "launches_solve_then_vjp_jvp_per_setting": counts, "fallback_count_lsqr_lsmr": fallbacks,
+                              "solved": int((sol.status == 1).sum())}), flush=True)
 
 
 def timing(reps=200):
