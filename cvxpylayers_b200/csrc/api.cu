@@ -82,6 +82,11 @@ struct Handle {
   Plan fwd_fast;    // fast_fwd: dense A, polyhedral cones, direct mode: register-tiled forward (fwd_fast.cu)
   int fast_fwd = 0;
   LsPlans ls[2];
+  // solution polishing (polish.cu): planned only for zero + nonneg cones, n <= 128, when it fits; otherwise polish_why says why
+  Plan polish;
+  int polish_ok = 0;
+  long long polish_stage = 0;   // doubles of its staging buffer (live rows of A, then W and S)
+  std::string polish_why;
   int small_mode = 1;   // BCONE_SMALL_CTA: 0 disables the 4-CTA/SM builds, 2 forces them
   // Per-stream scratch slabs (one per CTA of the grid): launches on different streams may overlap, launches on one
   // stream cannot, so the stream is the unit of ownership.  Allocated on first use.
@@ -364,6 +369,30 @@ int plan_backward(Handle *h, const Limits &L, int lsmr) {
   return rc;
 }
 
+// Solution polishing: zero + nonneg cones (a finite active set) and n <= 128 (W = L^{-1} A_L' is formed with 8 rows of A in a
+// warp's registers).  The staging buffer holds the live rows (at most min(m, n)), then W and S; it is as large as that needs
+// or as what is left of the opt-in shared memory, and an instance whose W and S do not fit it is not attempted.  Sets
+// h->polish_ok, or h->polish_why.  Never fails bcone_create.
+void plan_polish(Handle *h, const Limits &L) {
+  const DevStruct &S = h->S;
+  const int n = S.n, m = S.m;
+  if (S.ncones > 0 || S.ep + S.ed > 0) { h->polish_why = "polish: only structures with zero and nonneg cones have a finite active set to polish (this one has SOC, PSD or exponential cones)"; return; }
+  if (n > 128) { h->polish_why = "polish: needs n <= 128 (n = " + std::to_string(n) + ")"; return; }
+  const long long k = std::min(m, n), full = k * n + k * (k + 1) / 2;
+  for (int tt = L.threads; tt >= 128; tt /= 2) {
+    const size_t base = bc_polish_smem_bytes(n, m, tt, 0);
+    if (base > L.smem_cap) continue;
+    const long long cap = std::min(full, (long long)((L.smem_cap - base) / sizeof(double)) & ~1LL);
+    if (cap < std::min(full, (long long)n + 1)) continue;   // (not even one live row)
+    h->polish = Plan{bc_polish_kernel(S.dense), tt, bc_polish_smem_bytes(n, m, tt, cap)};
+    if (configure(h->polish) != cudaSuccess) { h->polish_why = "polish: kernel configuration failed"; return; }
+    h->polish_ok = 1; h->polish_stage = cap;
+    return;
+  }
+  h->polish_why = "polish: does not fit in shared memory (" + std::to_string(bc_polish_smem_bytes(n, m, 128, std::min(full, (long long)n + 1))) +
+                  " B needed, " + std::to_string(L.smem_cap) + " B per CTA available)";
+}
+
 // With values and vectors off chip, what is left in shared memory is the per-CTA scratch: the cone scratch (per-warp PSD
 // scratch, persistent eigenvectors, exp-cone slots) and the 8 n column partials.  Name the largest PSD order that would fit.
 std::string explain_no_fit(const Handle *h, const bcone_desc *d, size_t smem_cap) {
@@ -422,6 +451,7 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
   // A structure without an LSMR adjoint or without a forward-mode geometry (either method) is still accepted; only the calls
   // that need them refuse it.
   plan_backward(h, L, 1);
+  plan_polish(h, L);
   cudaGetLastError();   // (a refused configuration is not an error of this call)
   *out = h;
   return BCONE_OK;
@@ -902,6 +932,44 @@ extern "C" int bcone_jvp_shared(void *handle, int32_t B, const double *A_vals, c
                                 const double *db, const double *dc, double *dx, double *dy, double *ds, int32_t *lsqr_iters,
                                 const bcone_settings *stg, void *stream) {
   return jvp_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, dA, dP, db, dc, dx, dy, ds, lsqr_iters, 1, stg, stream);
+}
+
+// shared: A_vals [nnzA] / P_vals [nnzP] one copy for the batch
+static int polish_impl(Handle *h, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c, double *x,
+                       double *y, double *s, const int32_t *status, int32_t *polished, double *resid, int shared, const bcone_settings *stg,
+                       void *stream) {
+  if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !status || !polished || !stg) return fail(h, BCONE_EINVAL, "polish: null argument");
+  if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "polish: structure has P but P_vals is NULL");
+  if (!h->polish_ok) return fail(h, BCONE_EUNSUPPORTED, h->polish_why);
+  cudaStream_t st = (cudaStream_t)stream;
+  CK(cudaSetDevice(h->device), "polish set device");
+  PolishArgs a;
+  a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
+  a.x = x; a.y = y; a.s = s; a.status = status; a.polished = polished; a.resid = resid;
+  a.sA = shared ? 0 : h->S.nnzA; a.sP = shared ? 0 : h->S.nnzP;
+  a.use_tma = h->S.dense && (h->S.n % 2) == 0 && (((uintptr_t)A_vals & 15) == 0);
+  a.stage_cap = h->polish_stage;
+  a.delta = 1e-6; a.refine = 3;   // OSQP's defaults
+  int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
+  a.counter = ctr;
+  CK(cudaMemsetAsync(ctr, 0, sizeof(int), st), "polish counter");
+  CK(launch(h->polish, grid_for(h->polish, B, h->num_sms), &a, st), "polish launch");
+  h->launches++;
+  return BCONE_OK;
+}
+extern "C" int bcone_polish_supported(void *handle) {
+  Handle *h = (Handle *)handle;
+  if (!h) return BCONE_EINVAL;
+  return h->polish_ok ? BCONE_OK : fail(h, BCONE_EUNSUPPORTED, h->polish_why);
+}
+extern "C" int bcone_polish(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c, double *x,
+                            double *y, double *s, const int32_t *status, int32_t *polished, double *resid, const bcone_settings *st, void *stream) {
+  return polish_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, status, polished, resid, 0, st, stream);
+}
+extern "C" int bcone_polish_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                                   double *x, double *y, double *s, const int32_t *status, int32_t *polished, double *resid,
+                                   const bcone_settings *st, void *stream) {
+  return polish_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, status, polished, resid, 1, st, stream);
 }
 
 // Strided host<->device copy on the caller's stream (cudaMemcpy2DAsync): lets the reference-facing

@@ -113,6 +113,23 @@ struct BwdArgs {
   double *srec;
 };
 
+// Solution polishing (polish.cu, bcone_polish): x, y, s are read and, for an accepted instance, overwritten in place.
+struct PolishArgs {
+  DevStruct S;
+  int B;
+  const double *A_vals, *P_vals, *b, *c;
+  double *x, *y, *s;
+  const int *status;
+  int *polished;         // [B]: 1 accepted, 0 rejected (input kept), -1 not attempted
+  double *resid;         // [B,3] or NULL: rp, rd, gap of an accepted instance
+  long long sA, sP;      // batch strides of A_vals / P_vals (0: one copy shared by the batch)
+  int *counter;
+  int use_tma;           // dense A, n even, A_vals 16-byte aligned: live rows staged by TMA bulk copies
+  long long stage_cap;   // doubles of the buffer the live rows, W and S share
+  double delta;          // regularisation, relative to the largest absolute entry of P and A_L
+  int refine;            // iterative refinement steps
+};
+
 // Per-instance record of the shared-matrix adjoint: [r_x n | r_y m | r_tau | pi_y m].
 __host__ __device__ inline long long bc_srec_doubles(int n, int m) { return (long long)n + 2LL * m + 1; }
 // Written by the whole block; rx / ry / piy in shared memory (rx and ry may be one vector X = [r_x ; r_y ; r_tau]).
@@ -1619,6 +1636,9 @@ const void *bc_bwdb_kernel(int lsmr);
 const void *bc_lsmr_kernel(int dense, int small_cta, int jvp, int vals_global);
 const void *bc_bwdf_lsmr_kernel(int n);
 const void *bc_bwdb_lsmr_kernel(void);
+// polish.cu
+size_t bc_polish_smem_bytes(int n, int m, int threads, long long stage_cap);
+const void *bc_polish_kernel(int dense);
 // pack.cu
 cudaError_t bc_b2e(const double *in, double *out, int K, int B, int ldo, int roff, const int *smap, const int *dmap, double sign, long long ldb,
                    cudaStream_t st);

@@ -26,7 +26,8 @@ _ARG_MAP = {
     "lsqr_iter_lim": "lsqr_iter_lim", "lsqr_precond": "lsqr_precond", "adaptive_check": "adaptive_check",
     "acceleration_lookback": "acceleration_lookback", "acceleration_interval": "acceleration_interval",
 }
-_IGNORED = {"verbose", "n_jobs_forward", "n_jobs_backward", "solve_method", "warm_starts", "raise_on_error", "warm_start", "reuse_setup", "shared_matrices"}   # (warm_start / reuse_setup / shared_matrices are handled by the layer)
+_IGNORED = {"verbose", "n_jobs_forward", "n_jobs_backward", "solve_method", "warm_starts", "raise_on_error", "warm_start", "reuse_setup", "shared_matrices",
+            "polish"}   # (warm_start / reuse_setup / shared_matrices / polish are handled by the layer)
 
 
 def make_settings(args: dict | None) -> _lib.BconeSettings:
@@ -421,3 +422,37 @@ class Engine:
                 _ptr(dx), _ptr(dy), _ptr(ds), _ptr(its), C.byref(settings), self._stream())
         self._raise(rc, "bcone_jvp_shared" if shared else "bcone_jvp")
         return dx, dy, ds, its
+
+    def require_polish(self) -> None:
+        """Raise ValueError (naming the reason) unless the structure has a polish plan (``bcone_polish_supported``); no device work,
+        so a layer can refuse the option before it solves anything."""
+        if self.lib.bcone_polish_supported(self.h) != 0:
+            raise ValueError(self.lib.bcone_last_error(self.h).decode())
+
+    def polish(self, A_vals, b, c, sol: Solution, P_vals=None, settings: _lib.BconeSettings | None = None) -> torch.Tensor:
+        """Polish ``sol`` in place (``bcone_polish``, include/bcone.h): for each SOLVED / INACCURATE instance solve the KKT system
+        of the active set its iterate identifies and keep the result only where no residual (primal, dual, gap) grows; ``sol.resid``
+        is updated for those.  Statuses are not changed.  Returns polished[B] (int32): 1 accepted, 0 rejected (input kept),
+        -1 not attempted.  1-D ``A_vals[nnzA]`` (and ``P_vals[nnzP]``): one copy shared by the batch (``bcone_polish_shared``).
+        Structures with other than zero and nonneg cones, or n > 128, raise ValueError."""
+        st, dev, f64 = self.structure, self.device, torch.float64
+        shared = A_vals.dim() == 1
+        B = b.shape[0] if shared else A_vals.shape[0]
+        lead = () if shared else (B,)
+        for name, t, shp in (("A_vals", A_vals, (*lead, st.nnzA)), ("b", b, (B, st.m)), ("c", c, (B, st.n)),
+                             ("x", sol.x, (B, st.n)), ("y", sol.y, (B, st.m)), ("s", sol.s, (B, st.m))):
+            _chk(t, shp, f64, dev, name)
+        _chk(sol.status, (B,), torch.int32, dev, "status")
+        _chk(sol.resid, (B, 3), f64, dev, "resid")
+        if st.nnzP:
+            if P_vals is None:
+                raise ValueError("structure has a quadratic term but P_vals is None")
+            _chk(P_vals, (*lead, st.nnzP), f64, dev, "P_vals")
+        self.require_polish()
+        settings = settings or _lib.default_settings()
+        flags = torch.empty(B, dtype=torch.int32, device=dev)
+        fn = self.lib.bcone_polish_shared if shared else self.lib.bcone_polish
+        rc = fn(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c), _ptr(sol.x), _ptr(sol.y),
+                _ptr(sol.s), _ptr(sol.status), _ptr(flags), _ptr(sol.resid), C.byref(settings), self._stream())
+        self._raise(rc, "bcone_polish_shared" if shared else "bcone_polish")
+        return flags

@@ -323,7 +323,8 @@ def _side_streams(eng: Engine, dev):
     return ss
 
 
-def _forward_pipelined(eng: Engine, dev, A_eval, q_eval, P_eval, settings, use_P, warm=None, cache=None, staged: bool = False):
+def _forward_pipelined(eng: Engine, dev, A_eval, q_eval, P_eval, settings, use_P, warm=None, cache=None, staged: bool = False,
+                       polish: bool = False):
     st = eng.structure
     B = A_eval.shape[1]
     cstride = (cache.numel() // B) if cache is not None else 0
@@ -379,14 +380,14 @@ def _forward_pipelined(eng: Engine, dev, A_eval, q_eval, P_eval, settings, use_P
             return out
 
         futs = [sg.pool.submit(stage, k, lo, hi) for k, (lo, hi) in enumerate(chunks)]
-    for k, (lo, hi) in enumerate(chunks):
-        with torch.cuda.stream(streams[k % 2]):
-            Bc = hi - lo
-            A_c = torch.empty((A_eval.shape[0], Bc), dtype=f64, device=dev)
-            q_c = torch.empty((q_eval.shape[0], Bc), dtype=f64, device=dev)
-            P_c = torch.empty((P_eval.shape[0], Bc), dtype=f64, device=dev) if use_P else None
-            if staged:
-                try:
+    try:   # any exception leaving the chunk loop (a failed copy, solve or polish) releases the stager
+        for k, (lo, hi) in enumerate(chunks):
+            with torch.cuda.stream(streams[k % 2]):
+                Bc = hi - lo
+                A_c = torch.empty((A_eval.shape[0], Bc), dtype=f64, device=dev)
+                q_c = torch.empty((q_eval.shape[0], Bc), dtype=f64, device=dev)
+                P_c = torch.empty((P_eval.shape[0], Bc), dtype=f64, device=dev) if use_P else None
+                if staged:
                     hA_, hq_, hP_ = futs[k].result()
                     A_c.copy_(hA_, non_blocking=True)
                     q_c.copy_(hq_, non_blocking=True)
@@ -395,22 +396,25 @@ def _forward_pipelined(eng: Engine, dev, A_eval, q_eval, P_eval, settings, use_P
                     cev[k] = torch.cuda.Event()
                     cev[k].record(streams[k % 2])
                     enq[k].set()
-                except BaseException:
-                    abort.set()
-                    raise
-            else:
-                eng.copy2d(A_c, A_eval, lo, hi, True)
-                eng.copy2d(q_c, q_eval, lo, hi, True)
-                if use_P:
-                    eng.copy2d(P_c, P_eval, lo, hi, True)
-            eng.ingest(A_c, q_c, P_c, out=(A_vals[lo:hi], P_vals[lo:hi] if use_P else None, b[lo:hi], c[lo:hi]))
-            from .engine import Solution  # noqa: PLC0415
-            eng.solve(A_vals[lo:hi], b[lo:hi], c[lo:hi], P_vals[lo:hi] if use_P else None, settings,
-                      out=Solution(sol.x[lo:hi], sol.y[lo:hi], sol.s[lo:hi], sol.status[lo:hi], sol.iters[lo:hi], sol.resid[lo:hi]),
-                      warm=None if warm is None else tuple(w_[lo:hi] for w_ in warm),
-                      cache=None if cache is None else cache[lo * cstride:hi * cstride], reuse=True)
-            primal[lo:hi].copy_(sol.x[lo:hi], non_blocking=True)
-            dual[lo:hi].copy_(sol.y[lo:hi], non_blocking=True)
+                else:
+                    eng.copy2d(A_c, A_eval, lo, hi, True)
+                    eng.copy2d(q_c, q_eval, lo, hi, True)
+                    if use_P:
+                        eng.copy2d(P_c, P_eval, lo, hi, True)
+                eng.ingest(A_c, q_c, P_c, out=(A_vals[lo:hi], P_vals[lo:hi] if use_P else None, b[lo:hi], c[lo:hi]))
+                from .engine import Solution  # noqa: PLC0415
+                sol_c = Solution(sol.x[lo:hi], sol.y[lo:hi], sol.s[lo:hi], sol.status[lo:hi], sol.iters[lo:hi], sol.resid[lo:hi])
+                eng.solve(A_vals[lo:hi], b[lo:hi], c[lo:hi], P_vals[lo:hi] if use_P else None, settings, out=sol_c,
+                          warm=None if warm is None else tuple(w_[lo:hi] for w_ in warm),
+                          cache=None if cache is None else cache[lo * cstride:hi * cstride], reuse=True)
+                if polish:
+                    eng.polish(A_vals[lo:hi], b[lo:hi], c[lo:hi], sol_c, P_vals[lo:hi] if use_P else None, settings)
+                primal[lo:hi].copy_(sol.x[lo:hi], non_blocking=True)
+                dual[lo:hi].copy_(sol.y[lo:hi], non_blocking=True)
+    except BaseException:
+        if staged:
+            abort.set()   # (the stager must not wait for a slice that will never be copied)
+        raise
     for s_ in streams:
         cur.wait_stream(s_)
     return A_vals, P_vals, b, c, sol, primal, dual
@@ -484,14 +488,22 @@ class _CvxpyLayer(torch.autograd.Function):
         piped = _pipe_ok(eng, batch_size, A_eval.detach(), q_eval.detach(), P_eval.detach() if use_P else None)
         staged = (not piped) and eng.kernel_info()["fwd_smem"] > 0 and _stage_ok(batch_size, A_eval, q_eval, P_eval if use_P else None)
         piped = piped or staged
+        # polish: the solution is polished right after the solve, so the backward, the forward mode and the next warm start all
+        # see the polished point
+        polish = bool(merged.get("polish"))
+        if polish:
+            eng.require_polish()   # (before any chunk is staged or solved)
         with torch.cuda.device(dev):
             if piped:
                 A_vals, P_vals, b, c, sol, primal, dual = _forward_pipelined(
-                    eng, dev, A_eval.detach(), q_eval.detach(), P_eval.detach() if use_P else None, settings, use_P, warm, cache, staged)
+                    eng, dev, A_eval.detach(), q_eval.detach(), P_eval.detach() if use_P else None, settings, use_P, warm, cache, staged,
+                    polish)
             else:
                 A_vals, P_vals, b, c = eng.ingest(_to_dev(A_eval, dev), _to_dev(q_eval, dev),
                                                   _to_dev(P_eval, dev) if use_P else None)
                 sol = eng.solve(A_vals, b, c, P_vals, settings, warm=warm, cache=cache, reuse=True)
+                if polish:
+                    eng.polish(A_vals, b, c, sol, P_vals, settings)
             status = sol.status.cpu()  # the one host sync of the forward: per-instance status
         ctx.remember(dev, batch_size, sol, merged, warm_start)
         bad = (status != 1) & (status != 2)
@@ -622,10 +634,14 @@ class _CvxpyLayerFused(torch.autograd.Function):
         # shared_matrices: the caller states that A and P are the same for every instance (their parameters are unbatched);
         # they are evaluated once and the batch shares them through solve, adjoint and forward mode
         shared = bool(merged.get("shared_matrices"))
+        if merged.get("polish"):
+            eng.require_polish()
         with torch.cuda.device(dev):
             cache = ctx.setup_cache(eng, dev, B, merged)
             A_vals, P_vals, b, c = eng.ingest_params(_to_dev(ps, dev), shared=shared)
             sol = eng.solve(A_vals, b, c, P_vals, settings, warm=ctx.warm_for(dev, B, warm_start, merged), cache=cache, reuse=True)
+            if merged.get("polish"):   # (before the solution is kept for the backward, the forward mode and the next warm start)
+                eng.polish(A_vals, b, c, sol, P_vals, settings)
             status = sol.status.cpu()
         ctx.remember(dev, B, sol, merged, warm_start)
         bad = (status != 1) & (status != 2)

@@ -262,6 +262,30 @@ int bcone_path_info(void *handle, int32_t *fwd_path, int32_t *bwd_path);
  * that build takes it. */
 int bcone_small_cta_info(void *handle, int32_t *fwd_small_ctas, int32_t *bwd_small_ctas);
 
+/* Solution polishing (OSQP's `polish`) for QPs and LPs whose cones are zero and nonneg only, n <= 128.  For every instance
+ * whose status is SOLVED (1) or INACCURATE (2): the live rows L are the zero rows and the nonneg rows with y_i > s_i; the
+ * equality-constrained QP of L is solved through [[P + d I, A_L'], [A_L, -d I]] (d = 1e-6 x the largest absolute entry of P
+ * and A_L) and three steps of iterative refinement against the unregularised KKT matrix; the point is completed with y = 0
+ * off L, s = b - A x and s_L = 0, and s, y clipped at 0 on the nonneg rows.  It replaces the input only when none of
+ * rp = |Ax + s - b|_inf, rd = |Px + A'y + c|_inf, gap = |x'Px + c'x + b'y| exceeds the input's.  THE STATUS IS NEVER CHANGED.
+ *   x[B,n], y[B,m], s[B,m]: read, and overwritten for accepted instances only (a rejected one keeps its bits);
+ *   status[B]: the forward's; polished[B] (int32, out): 1 accepted, 0 rejected (input kept; also when P + d I or the Schur
+ *   complement is not positive definite), -1 not attempted (other status, a non-finite x / y / s, or more live rows than
+ *   n or than the staging buffer holds); resid[B,3] or NULL: rp, rd, gap, updated for accepted instances.  `st` is taken for
+ *   symmetry with the other entry points; polishing has no setting (d and the refinement count are fixed).
+ * No atomics: results are deterministic.  BCONE_EUNSUPPORTED (message: the cone types, n, or the shared memory) for a
+ * structure without a polish plan.  bcone_polish_shared: A_vals[nnzA] / P_vals[nnzP] one copy for the batch; the same bits
+ * as bcone_polish on the expanded copies. */
+int bcone_polish(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                 double *x, double *y, double *s, const int32_t *status, int32_t *polished, double *resid,
+                 const bcone_settings *st, void *cuda_stream);
+/* BCONE_OK when the structure has a polish plan, else BCONE_EUNSUPPORTED with the reason in bcone_last_error(handle): lets a
+ * caller refuse the option before it solves anything.  No device work. */
+int bcone_polish_supported(void *handle);
+int bcone_polish_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                        double *x, double *y, double *s, const int32_t *status, int32_t *polished, double *resid,
+                        const bcone_settings *st, void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
