@@ -87,6 +87,10 @@ struct Handle {
   int polish_ok = 0;
   long long polish_stage = 0;   // doubles of its staging buffer (live rows of A, then W and S)
   std::string polish_why;
+  // solution refinement (refine.cu): the forward mode's tiers with the refinement kernel's sizes; refine_why when it does not fit
+  TieredPlan refine;
+  int refine_ok = 0, refine_last_small = -1;   // (the build the last bcone_refine launch took: bcone_refine_info)
+  std::string refine_why;
   int small_mode = 1;   // BCONE_SMALL_CTA: 0 disables the 4-CTA/SM builds, 2 forces them
   // Per-stream scratch slabs (one per CTA of the grid): launches on different streams may overlap, launches on one
   // stream cannot, so the stream is the unit of ownership.  Allocated on first use.
@@ -94,7 +98,7 @@ struct Handle {
   // srec / part = the adjoint's per-instance r, pi_y records and the reduction's partial sums (shared.cu)
   // bwd / jvp: the generic backward's vector slabs, per least-squares method
   struct StreamWs { cudaStream_t s; double *fwd = nullptr, *aa = nullptr, *park = nullptr; size_t aa_cap = 0;
-                    double *bwd[2] = {nullptr, nullptr}, *jvp[2] = {nullptr, nullptr};
+                    double *bwd[2] = {nullptr, nullptr}, *jvp[2] = {nullptr, nullptr}, *refine = nullptr;
                     double *setup = nullptr, *srec = nullptr, *part = nullptr; size_t srec_cap = 0, part_cap = 0; };
   std::vector<StreamWs> sws;
   int *fail_list[RING] = {nullptr}; int fail_cap[RING] = {0};
@@ -312,25 +316,32 @@ int plan_forward(Handle *h, const Limits &L) {
   return BCONE_OK;
 }
 
-// Generic LSQR kernel (bwd.cu), as the adjoint or as the forward mode, or its LSMR variant (lsmr = 1): prefer P staged in
-// shared memory, then vectors on chip, then vectors in L2; values off chip last.  BCONE_OK, BCONE_EUNSUPPORTED (no tier fits)
-// or BCONE_ECUDA (message set).
-int plan_lsqr(Handle *h, const Limits &L, TieredPlan &t, int jvp, int lsmr) {
+// Generic LSQR kernel (bwd.cu), as the adjoint or as the forward mode, or its LSMR variant (lsmr = 1), or the refinement
+// kernel (refine = 1: the forward mode's kernel with the refinement's vectors, refine.cu): prefer P staged in shared memory, then
+// vectors on chip, then vectors in L2; values off chip last.  BCONE_OK, BCONE_EUNSUPPORTED (no tier fits) or BCONE_ECUDA
+// (message set).
+int plan_lsqr(Handle *h, const Limits &L, TieredPlan &t, int jvp, int lsmr, int refine = 0) {
   const DevStruct &S = h->S;
   const int npoly = S.z + S.l;
+  auto smem = [&](int psm, int tt, int vg, int vals) {
+    const int nnzP = psm ? S.nnzP : 0, nexp = S.ep + S.ed;
+    return refine ? bc_refine_smem_bytes(S.n, S.m, npoly, S.nnzA, nnzP, tt, S.max_psd, h->psd_total, nexp, vg, vals)
+                  : bc_bwd_smem_bytes(S.n, S.m, npoly, S.nnzA, nnzP, tt, S.max_psd, h->psd_total, nexp, vg, vals, lsmr);
+  };
+  auto kernel = [&](int small) { return refine ? bc_refine_kernel(S.dense, small, t.vals_global) : bc_lsqr_kernel(S.dense, small, jvp, t.vals_global, lsmr); };
   for (int vals = L.vals_lo; vals <= 1 && !t.big.threads; vals++)
     for (int vg = 0; vg <= 1 && !t.big.threads; vg++)
       for (int psm = (S.nnzP > 0 ? 1 : 0); psm >= 0 && !t.big.threads; psm--)
         for (int tt = L.threads; tt >= 64; tt /= 2) {
-          size_t sm = bc_bwd_smem_bytes(S.n, S.m, npoly, S.nnzA, psm ? S.nnzP : 0, tt, S.max_psd, h->psd_total, S.ep + S.ed, vg, vals, lsmr);
+          size_t sm = smem(psm, tt, vg, vals);
           if (sm <= L.smem_cap) { t.big.threads = tt; t.big.smem = sm; t.p_in_smem = psm; t.vec_global = vg; t.vals_global = vals; break; }
           if (psm) break;  // do not trade threads for P residency
         }
   if (!t.big.threads) return BCONE_EUNSUPPORTED;
-  t.big.fn = bc_lsqr_kernel(S.dense, 0, jvp, t.vals_global, lsmr);
-  const cudaError_t e = configure_tiers(h, t, bc_lsqr_kernel(S.dense, 1, jvp, t.vals_global, lsmr));
+  t.big.fn = kernel(0);
+  const cudaError_t e = configure_tiers(h, t, kernel(1));
   if (e != cudaSuccess) return cuda_fail(nullptr, e, "cudaFuncSetAttribute");
-  if (t.vec_global) t.ws_stride = bc_bwd_ws_doubles(S.n, S.m, npoly, lsmr);
+  if (t.vec_global) t.ws_stride = refine ? bc_refine_ws_doubles(S.n, S.m, npoly) : bc_bwd_ws_doubles(S.n, S.m, npoly, lsmr);
   return BCONE_OK;
 }
 
@@ -393,6 +404,15 @@ void plan_polish(Handle *h, const Limits &L) {
                   " B needed, " + std::to_string(L.smem_cap) + " B per CTA available)";
 }
 
+// Solution refinement: the forward mode's tier search with the refinement kernel's sizes (every cone type has one).  Sets
+// h->refine_ok, or h->refine_why.  Never fails bcone_create: refinement is optional like the forward-mode plans.
+void plan_refine(Handle *h, const Limits &L) {
+  const int rc = plan_lsqr(h, L, h->refine, 1, 0, 1);
+  h->refine_ok = rc == BCONE_OK;
+  if (rc == BCONE_EUNSUPPORTED) h->refine_why = "refine: the instance does not fit the refinement kernel, even with the values and vectors in global memory";
+  else if (rc != BCONE_OK) h->refine_why = "refine: kernel configuration failed (" + g_create_err + ")";
+}
+
 // With values and vectors off chip, what is left in shared memory is the per-CTA scratch: the cone scratch (per-warp PSD
 // scratch, persistent eigenvectors, exp-cone slots) and the 8 n column partials.  Name the largest PSD order that would fit.
 std::string explain_no_fit(const Handle *h, const bcone_desc *d, size_t smem_cap) {
@@ -452,6 +472,7 @@ extern "C" int bcone_create(const bcone_desc *d, void **out) {
   // that need them refuse it.
   plan_backward(h, L, 1);
   plan_polish(h, L);
+  plan_refine(h, L);
   cudaGetLastError();   // (a refused configuration is not an error of this call)
   *out = h;
   return BCONE_OK;
@@ -970,6 +991,71 @@ extern "C" int bcone_polish_shared(void *handle, int32_t B, const double *A_vals
                                    double *x, double *y, double *s, const int32_t *status, int32_t *polished, double *resid,
                                    const bcone_settings *st, void *stream) {
   return polish_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, status, polished, resid, 1, st, stream);
+}
+
+// shared: A_vals [nnzA] / P_vals [nnzP] one copy for the batch
+static int refine_impl(Handle *h, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c, double *x,
+                       double *y, double *s, const int32_t *status, int32_t *refined, double *resid, int32_t steps, int shared,
+                       const bcone_settings *stg, void *stream) {
+  if (!h || B <= 0 || !A_vals || !b || !c || !x || !y || !s || !status || !refined || !stg) return fail(h, BCONE_EINVAL, "refine: null argument");
+  if (h->S.nnzP > 0 && !P_vals) return fail(h, BCONE_EINVAL, "refine: structure has P but P_vals is NULL");
+  if (steps < 1 || steps > 10) return fail(h, BCONE_EINVAL, "refine: steps must be 1 ... 10 (got " + std::to_string(steps) + ")");
+  if (!h->refine_ok) return fail(h, BCONE_EUNSUPPORTED, h->refine_why);
+  const TieredPlan &gen = h->refine;
+  cudaStream_t st = (cudaStream_t)stream;
+  RefineArgs ra{};
+  BwdArgs &a = ra.a;
+  a.S = h->S; a.B = B; a.A_vals = A_vals; a.P_vals = h->S.nnzP > 0 ? P_vals : nullptr; a.b = b; a.c = c;
+  a.x = x; a.y = y; a.s = s; a.tx = x; a.ty = y; a.ts = s;
+  a.sA = shared ? 0 : h->S.nnzA; a.sP = shared ? 0 : h->S.nnzP;
+  int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
+  a.st = kernel_settings(*stg); a.counter = ctr + 1;
+  if (a.st.lsqr_precond == 2) a.st.lsqr_precond = 1;   // (as for the forward mode)
+  a.use_tma = gen.vals_global || (h->tma_ok && (((uintptr_t)A_vals & 15) == 0)); a.psd_total = h->psd_total; a.p_in_smem = gen.p_in_smem;
+  ra.status = status; ra.flags = refined; ra.resid = resid; ra.steps = steps;
+  CK(cudaSetDevice(h->device), "refine set device");
+  a.ws_stride = (long long)gen.ws_stride;
+  if (gen.vec_global) {
+    Handle::StreamWs *sw = stream_ws(h, st);
+    if (!ensure_slab(h, &sw->refine, nullptr, gen.ws_stride * max_grid(gen, h->num_sms))) return fail(h, BCONE_ENOMEM, "cudaMalloc refine workspace");
+    a.ws = sw->refine;
+  }
+  a.prof = h->prof;
+  CK(cudaMemsetAsync(ctr + 1, 0, sizeof(int), st), "refine counter");
+  const Plan &plan = pick(gen, B, h->num_sms, h->small_mode);
+  h->refine_last_small = &plan == &gen.small;
+  CK(launch(plan, grid_for(plan, B, h->num_sms), &ra, st), "refine launch");
+  h->launches++;
+  return BCONE_OK;
+}
+extern "C" int bcone_refine_supported(void *handle) {
+  Handle *h = (Handle *)handle;
+  if (!h) return BCONE_EINVAL;
+  return h->refine_ok ? BCONE_OK : fail(h, BCONE_EUNSUPPORTED, h->refine_why);
+}
+extern "C" int bcone_refine_info(void *handle, int32_t *threads, int32_t *ctas_per_sm, int32_t *small_ctas_per_sm, int32_t *vals_global,
+                                 int32_t *vec_global, int32_t *num_sms, int32_t *last_small) {
+  Handle *h = (Handle *)handle;
+  if (!h) return BCONE_EINVAL;
+  const TieredPlan &t = h->refine;
+  if (threads) *threads = h->refine_ok ? t.big.threads : 0;
+  if (ctas_per_sm) *ctas_per_sm = h->refine_ok ? t.big.ctas : 0;
+  if (small_ctas_per_sm) *small_ctas_per_sm = h->refine_ok && t.has_small ? t.small.ctas : 0;
+  if (vals_global) *vals_global = t.vals_global;
+  if (vec_global) *vec_global = t.vec_global;
+  if (num_sms) *num_sms = h->num_sms;
+  if (last_small) *last_small = h->refine_last_small;
+  return BCONE_OK;
+}
+extern "C" int bcone_refine(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c, double *x,
+                            double *y, double *s, const int32_t *status, int32_t *refined, double *resid, int32_t steps, const bcone_settings *st,
+                            void *stream) {
+  return refine_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, status, refined, resid, steps, 0, st, stream);
+}
+extern "C" int bcone_refine_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                                   double *x, double *y, double *s, const int32_t *status, int32_t *refined, double *resid, int32_t steps,
+                                   const bcone_settings *st, void *stream) {
+  return refine_impl((Handle *)handle, B, A_vals, P_vals, b, c, x, y, s, status, refined, resid, steps, 1, st, stream);
 }
 
 // Strided host<->device copy on the caller's stream (cudaMemcpy2DAsync): lets the reference-facing

@@ -18,24 +18,25 @@ struct BwdSmem {
   int *ibuf;
 };
 
-// v is only kept for the non-polyhedral rows (nonneg rows use pi_y > 0 <=> v > 0 as their mask).  LSMR keeps one more N-vector.
-__host__ __device__ inline size_t bwd_vec_doubles(int n, int m, int npoly, int lsmr = 0) {
+// v is only kept for the non-polyhedral rows (nonneg rows use pi_y > 0 <=> v > 0 as their mask).  LSMR keeps one more N-vector,
+// solution refinement (refine.cu) the iterate x, v, its pi_y and the y rows of its residual.
+__host__ __device__ inline size_t bwd_vec_doubles(int n, int m, int npoly, int lsmr = 0, int refine = 0) {
   size_t N = (size_t)n + m + 1;
-  return 3 * (size_t)n + 2 * (size_t)m + (m - npoly) + (lsmr ? 8 : 7) * N + 2 * (size_t)m;
+  return 3 * (size_t)n + 2 * (size_t)m + (m - npoly) + (lsmr ? 8 : 7) * N + 2 * (size_t)m + (refine ? (size_t)n + 3 * (size_t)m : 0);
 }
 // vec_global: large instances keep the LSQR vectors in a per-CTA slab of global memory.
 // vals_global: the CSR values are read in place from the caller's A_vals (instances whose values do not fit on chip).
 __host__ __device__ inline size_t bwd_smem_doubles(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
-                                                   int vals_global, int lsmr = 0) {
+                                                   int vals_global, int lsmr = 0, int refine = 0) {
   size_t d = 4 + (vals_global ? 0 : ((size_t)nnzA + 1) & ~(size_t)1) + (((size_t)nnzP_smem + 1) & ~(size_t)1) + threads + 2 * 32;
-  if (!vec_global) d += bwd_vec_doubles(n, m, npoly, lsmr);
+  if (!vec_global) d += bwd_vec_doubles(n, m, npoly, lsmr, refine);
   if (max_psd > 0) d += psd_total + (size_t)(threads / 32) * (3 * (size_t)max_psd * max_psd + max_psd);
   return d + 9 * (size_t)nexp;
 }
 
 // VG: no shared memory for the values (M.Av is set per instance); LSMR: one more N-vector behind t2 (LSMR's h-bar; not a
-// member of BwdSmem, whose layout the LSQR kernels' code depends on)
-template <bool VG = false, bool LSMR = false>
+// member of BwdSmem, whose layout the LSQR kernels' code depends on); REFINE: n + 3m doubles behind t2 (refine.cu)
+template <bool VG = false, bool LSMR = false, bool REFINE = false>
 __device__ __forceinline__ void carve_b(BwdSmem &M, double *base, double *gws, int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp) {
   const int N = n + m + 1;
   double *q = base;
@@ -53,6 +54,7 @@ __device__ __forceinline__ void carve_b(BwdSmem &M, double *base, double *gws, i
   M.Lsc = v; v += N; M.Rsc = v; v += N; M.tin = v; v += N;
   M.t1 = v; v += m; M.t2 = v; v += m;
   if (LSMR) v += N;
+  if (REFINE) v += n + 3 * m;
   if (!gws) q = v;
   M.expJ = q; q += 9 * nexp;
   M.psdVL = q; q += psd_total;
@@ -303,6 +305,68 @@ __device__ __noinline__ void jvp_inactive_rows(const BwdArgs &a, const BwdSmem &
   __syncthreads();
 }
 
+#ifdef BC_REFINE
+// Solution refinement (refine.cu): U <- -R at the point in x, pi_y (v = vw + alpha z_y on the polyhedral rows, M.v elsewhere),
+//   R = [P x + A' pi_y + c ;  b - A x - (pi_y - v) ;  -(x'P x + c'x + b'pi_y)],
+// the residual map of the homogeneous embedding at tau = 1.  Returns ||R||_2^2 (block-uniform).  W holds P x on the way.
+template <bool DENSE>
+__device__ __noinline__ double refine_rhs(const BwdArgs &a, const BwdSmem &M, const double *Pg, const double *vw, double alpha,
+                                          const ColPlan &plA, const ColPlan &plN) {
+  const DevStruct &S = a.S;
+  const int n = S.n, m = S.m, T = blockDim.x, t = threadIdx.x, npoly = S.z + S.l;
+  for (int j = t; j < n; j += T) M.W[j] = 0.0;
+  __syncthreads();
+  AT_mul<DENSE>(S, M.Av, M.piy, M.part, [&](int j, double v) { M.U[j] = -(v + M.c[j]); }, plA);
+  if (Pg) P_mul(S, Pg, M.x, M.part, [&](int j, double v) { M.W[j] += v; }, plN);
+  A_mul<DENSE>(S, M.Av, M.x, [&](int i, double v) {
+    const double vi = i >= npoly ? M.v[i] : fma(alpha, M.X[n + i], vw[i]);
+    M.U[n + i] = v + M.piy[i] - vi - M.b[i]; });
+  __syncthreads();
+  double d2[2] = {0, 0};   // tau component, ||R_x||^2 + ||R_y||^2
+  for (int j = t; j < n; j += T) {
+    const double w = M.W[j], u = M.U[j] - w;
+    M.U[j] = u; d2[0] = fma(M.x[j], w + M.c[j], d2[0]); d2[1] = fma(u, u, d2[1]);
+  }
+  for (int i = t; i < m; i += T) { const double u = M.U[n + i]; d2[0] = fma(M.b[i], M.piy[i], d2[0]); d2[1] = fma(u, u, d2[1]); }
+  block_reduce<2, false>(d2, M.red);
+  if (t == 0) M.U[n + m] = d2[0];
+  return fma(d2[0], d2[0], d2[1]);
+}
+
+// The equilibrated solve drops an inactive nonneg row's unknown with its equation (as for the forward mode, jvp_inactive_rows):
+// recover it from that equation, z_{n+i} = (A z_x)_i - R_{y,i}  (ryw = -R_y; the tau column is masked).  Ends with a barrier.
+template <bool DENSE>
+__device__ __noinline__ void refine_inactive_rows(const BwdArgs &a, const BwdSmem &M, const double *ryw) {
+  const DevStruct &S = a.S;
+  const int n = S.n, lo = S.z, hi = S.z + S.l;
+  A_mul<DENSE>(S, M.Av, M.X, [&](int i, double v) { if (i >= lo && i < hi && !(M.piy[i] > 0)) M.X[n + i] = v + ryw[i]; });
+  __syncthreads();
+}
+
+// Polishing's acceptance metrics of the point (x, y, s) (shared or global memory): rp = |A x + s - b|_inf,
+// rd = |P x + A'y + c|_inf, gap = |x'P x + c'x + b'y|; NaN counts as inf.  Block-uniform.  Uses V, W, t1.
+struct RefMet { double r[3]; };
+template <bool DENSE>
+__device__ __noinline__ RefMet refine_metrics(const BwdArgs &a, const BwdSmem &M, const double *Pg, const double *x, const double *y,
+                                              const double *s, const ColPlan &plA, const ColPlan &plN) {
+  const DevStruct &S = a.S;
+  const int n = S.n, m = S.m, T = blockDim.x, t = threadIdx.x;
+  __syncthreads();
+  for (int j = t; j < n; j += T) M.W[j] = 0.0;
+  A_mul<DENSE>(S, M.Av, x, [&](int i, double v) { M.t1[i] = v; });
+  AT_mul<DENSE>(S, M.Av, y, M.part, [&](int j, double v) { M.V[j] = v; }, plA);   // (ends synchronised)
+  if (Pg) P_mul(S, Pg, x, M.part, [&](int j, double v) { M.W[j] += v; }, plN);
+  __syncthreads();
+  auto amax = [](double acc, double v) { const double e = fabs(v); return e == e ? fmax(acc, e) : INFINITY; };
+  double mx[2] = {0, 0}, sm[1] = {0};
+  for (int i = t; i < m; i += T) { mx[0] = amax(mx[0], M.t1[i] + s[i] - M.b[i]); sm[0] = fma(M.b[i], y[i], sm[0]); }
+  for (int j = t; j < n; j += T) { mx[1] = amax(mx[1], M.W[j] + M.V[j] + M.c[j]); sm[0] = fma(x[j], M.W[j] + M.c[j], sm[0]); }
+  block_reduce<2, true>(mx, M.red);
+  block_reduce<1, false>(sm, M.red);
+  return RefMet{{mx[0], mx[1], fabs(sm[0])}};
+}
+#endif
+
 // JVP: the forward-mode derivative (bcone_jvp) instead of the adjoint -- the exact transpose of the map above:
 //   g  = [-dA' pi_y - dc - dP x ; dA x - db ; pi_y'db + x'dc + x'dP x]   (tangents dA, dP, db, dc read from global memory)
 //   z  = LSQR(M, g);  dx = z_x - x z_tau,  dy = D z_y - y z_tau,  ds = D z_y - z_y - s z_tau
@@ -312,26 +376,41 @@ __device__ __noinline__ void jvp_inactive_rows(const BwdArgs &a, const BwdSmem &
 // LSMR: diffcp's mode = "lsmr" (settings.lsmr = 1) -- LSMR (common.cuh lsmr_block) in place of LSQR on the same operator,
 // scalings and right-hand side.  bwd_lsmr.cu compiles this file again with BC_LSMR defined: the same kernels with LSMR, named
 // bwd_lsmr_kernel, in a translation unit of their own (so that the LSQR kernels compile to the code they had without them).
-#ifdef BC_LSMR
+// REFINE: solution refinement (bcone_refine) -- refine.cu compiles this file with BC_REFINE defined: the forward-mode kernel
+// (JVP = true) named refine_kernel, with the residual as its right-hand side, the tau column masked, a Newton loop with a
+// line search around set-up and LSQR, and its own write-back.
+#if defined(BC_REFINE)
+#define BWD_KERNEL refine_kernel
+constexpr bool LSMR = false, REFINE = true;
+#elif defined(BC_LSMR)
 #define BWD_KERNEL bwd_lsmr_kernel
-constexpr bool LSMR = true;
+constexpr bool LSMR = true, REFINE = false;
 #else
 #define BWD_KERNEL bwd_kernel
-constexpr bool LSMR = false;
+constexpr bool LSMR = false, REFINE = false;
 #endif
 template <bool DENSE, bool SMALL = false, bool JVP = false, bool VG = false>   // SMALL: <= 256 threads, four resident CTAs per SM (see fwd.cu)
+#ifdef BC_REFINE
+__global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(const __grid_constant__ RefineArgs ra) {
+  const BwdArgs &a = ra.a;
+#else
 __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(const __grid_constant__ BwdArgs a) {
+#endif
   extern __shared__ __align__(16) double smem[];
   const DevStruct &S = a.S;
   const int n = S.n, m = S.m, N = n + m + 1, T = blockDim.x, t = threadIdx.x;
   const bc_settings &st = a.st;
   BwdSmem M;
-  carve_b<VG, LSMR>(M, smem, a.ws ? a.ws + (size_t)blockIdx.x * a.ws_stride : nullptr, n, m, S.z + S.l, S.nnzA, a.p_in_smem ? S.nnzP : 0, T, S.max_psd,
+  carve_b<VG, LSMR, REFINE>(M, smem, a.ws ? a.ws + (size_t)blockIdx.x * a.ws_stride : nullptr, n, m, S.z + S.l, S.nnzA, a.p_in_smem ? S.nnzP : 0, T, S.max_psd,
               a.psd_total, S.ep + S.ed);
   if (t == 0) { mbar_init(M.bar, 1); fence_mbar_init(); }
   __syncthreads();
   uint32_t tma_phase = 0;
   const ColPlan plA = make_colplan(m, n), plN = make_colplan(n, n);
+#ifdef BC_REFINE
+  // the iterate w = (x, v): x, v, pi_y(v), and -R_y at w (the y rows of the last accepted right-hand side; later s)
+  double *const xw = M.t2 + m, *const vw = xw + n, *const yw = vw + m, *const ryw = yw + m;
+#endif
 
   for (;;) {
     if constexpr (LSMR) {   // (also the second pass of the block-preconditioned LSMR adjoint: the instances on its device-side list)
@@ -368,6 +447,40 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(c
     }
     if (Pglob && a.p_in_smem && !tmaP) for (int k = t; k < S.nnzP; k += T) M.Pv[k] = Pglob[k];
     const double *dxg = a.dx + (size_t)inst * n, *dyg = a.dy + (size_t)inst * m;
+#ifdef BC_REFINE
+    // ---- the input: status and finiteness, w = (x, y - s), its acceptance metrics ----
+    (void)dyg;
+    const double *xg = a.x + (size_t)inst * n, *yg = a.y + (size_t)inst * m, *sg = a.s + (size_t)inst * m;
+    bool finite = true;
+    for (int j = t; j < n; j += T) { const double v = xg[j]; xw[j] = v; M.c[j] = a.c[(size_t)inst * n + j]; finite &= isfinite(v); }
+    for (int i = t; i < m; i += T) {
+      const double yi = yg[i], si = sg[i];
+      vw[i] = yi - si; M.b[i] = a.b[(size_t)inst * m + i]; finite &= isfinite(yi) && isfinite(si);
+    }
+    for (int k = t; k < N; k += T) M.X[k] = 0.0;
+    if (VG ? tmaP : (bool)a.use_tma) { mbar_wait(M.bar, tma_phase); tma_phase ^= 1; }
+    finite = __syncthreads_and(finite);
+    const int stat = ra.status[inst];
+    if ((stat != 1 && stat != 2) || !finite) {
+      if (t == 0) ra.flags[inst] = -1;
+      continue;
+    }
+    const RefMet r0 = refine_metrics<DENSE>(a, M, Pg, xg, yg, sg, plA, plN);
+    // ---- Newton loop: each pass sets up the trial point w + alpha z (z = M.X; alpha = 0: the input) and takes its residual.
+    //      Accepted (the first point, or ||R|| below the iterate's): w <- trial, then LSQR for the next z.  Rejected: alpha halves
+    //      down to 1/32, then stop. ----
+    double alpha = 0.0, rn_w = 0.0;
+    int steps = 0;
+    bool have_w = false;
+    for (;;) {
+    for (int j = t; j < n; j += T) { M.x[j] = fma(alpha, M.X[j], xw[j]); M.px2c[j] = 0.0; }
+    for (int i = t; i < m; i += T) {
+      const double vi = fma(alpha, M.X[n + i], vw[i]);
+      if (i >= S.z + S.l) M.v[i] = vi;
+      M.piy[i] = (i >= S.z && i < S.z + S.l) ? fmax(vi, 0.0) : vi;
+    }
+    __syncthreads();
+#else
     for (int j = t; j < n; j += T) {
       M.x[j] = a.x[(size_t)inst * n + j]; M.c[j] = a.c[(size_t)inst * n + j]; M.px2c[j] = 0.0;
     }
@@ -381,6 +494,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(c
     }
     if (VG ? tmaP : (bool)a.use_tma) { mbar_wait(M.bar, tma_phase); tma_phase ^= 1; }
     __syncthreads();
+#endif
     // ---- cone Jacobian set-up: pi_y on SOC/PSD blocks, eigen-decompositions for PSD blocks ----
     if (S.ncones > 0) {
       const int lane = t & 31, warp = t >> 5, nw = T >> 5;
@@ -434,7 +548,23 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(c
     for (int j = t; j < n; j += T) M.px2c[j] = 2.0 * M.px2c[j] + M.c[j];
     double d3[3] = {0, 0, 0};
     if constexpr (JVP) {
+#ifdef BC_REFINE
+      const double rn = refine_rhs<DENSE>(a, M, Pg, vw, alpha, plA, plN);   // -R -> U (syncs px2c)
+      if (!have_w || rn < rn_w) {   // (NaN: rejected)
+        for (int j = t; j < n; j += T) xw[j] = M.x[j];
+        for (int i = t; i < m; i += T) { vw[i] = fma(alpha, M.X[n + i], vw[i]); yw[i] = M.piy[i]; ryw[i] = M.U[n + i]; }
+        rn_w = rn; have_w = true;
+        if (steps == ra.steps || !(rn > 0)) break;
+        steps++;
+        d3[1] = 1.0;
+      } else if ((alpha *= 0.5) < 1.0 / 32) {
+        break;
+      } else {
+        continue;
+      }
+#else
       d3[1] = jvp_rhs<DENSE>(a, M, inst, plA, plN);   // g -> U (syncs px2c)
+#endif
     } else {
       // ---- dz -> U ----
       apply_D(S, M, M.t1, M.t2);  // t2 = D dy   (also syncs px2c)
@@ -459,15 +589,29 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(c
       const double atol = st.lsqr_atol, btol = st.lsqr_btol;
       const double ctol = st.lsqr_conlim > 0 ? 1.0 / st.lsqr_conlim : 0.0;
       const int iter_lim = st.lsqr_iter_lim < 0 ? 2 * N : st.lsqr_iter_lim;
+#ifdef BC_REFINE
+      const bool pc = true;   // (the tau column is masked by a zero column scaling; lsqr_precond = 0: otherwise identity)
+#else
       const bool pc = st.lsqr_precond != 0;
+#endif
       // row / column scaling of B: the equilibration is computed for M', so M takes it with the two sides swapped
       // (an inactive nonneg row zeroes column n+i of M, which is e_{n+i}, and row n+i: see jvp_inactive_rows)
       double *const Ls = JVP ? M.Rsc : M.Lsc, *const Rs = JVP ? M.Lsc : M.Rsc;
+#ifdef BC_REFINE
+      if (st.lsqr_precond != 0) equilibrate<DENSE>(a, M, Pg, xPx, st.ruiz_passes > 0 ? st.ruiz_passes : 10, plA, plN);
+      for (int k = t; k < N; k += T) {
+        if (st.lsqr_precond == 0) { M.Lsc[k] = 1.0; M.Rsc[k] = 1.0; }
+        if (k == N - 1) M.Lsc[k] = 0.0;   // tau fixed at 1: its column of M is dropped
+        M.U[k] *= Ls[k]; M.X[k] = 0.0;
+      }
+      __syncthreads();
+#else
       if (pc) {
         equilibrate<DENSE>(a, M, Pg, xPx, st.ruiz_passes > 0 ? st.ruiz_passes : 10, plA, plN);
         for (int k = t; k < N; k += T) { M.U[k] *= Ls[k]; M.X[k] = 0.0; }
         __syncthreads();
       }
+#endif
       // B = diag(Lsc) M' diag(Rsc), or diag(Rsc) M diag(Lsc) for the JVP  (identity scalings when lsqr_precond = 0);
       // both products accumulate
       auto acc_B = [&](const double *in, double *out) {   // out += B in
@@ -576,9 +720,28 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(c
       }
 #endif
       if (pc) { __syncthreads(); for (int k = t; k < N; k += T) M.X[k] *= Rs[k]; }
+#ifdef BC_REFINE
+      if (st.lsqr_precond != 0 && S.l > 0) { __syncthreads(); refine_inactive_rows<DENSE>(a, M, ryw); }
+#else
       if constexpr (JVP) if (pc && S.l > 0) { __syncthreads(); jvp_inactive_rows<DENSE>(a, M, inst); }
+#endif
     }
     __syncthreads();
+#ifdef BC_REFINE
+    alpha = 1.0;
+    }   // (Newton loop)
+    // ---- write-back: the candidate (x, pi_y, pi_y - v) replaces the input only if none of rp, rd, gap grows ----
+    __syncthreads();
+    for (int i = t; i < m; i += T) ryw[i] = yw[i] - vw[i];
+    const RefMet r1 = refine_metrics<DENSE>(a, M, Pg, xw, yw, ryw, plA, plN);
+    const bool accept = r1.r[0] <= r0.r[0] && r1.r[1] <= r0.r[1] && r1.r[2] <= r0.r[2];   // (false for a NaN)
+    if (accept) {
+      for (int j = t; j < n; j += T) a.tx[(size_t)inst * n + j] = xw[j];
+      for (int i = t; i < m; i += T) { a.ty[(size_t)inst * m + i] = yw[i]; a.ts[(size_t)inst * m + i] = ryw[i]; }
+      if (t == 0 && ra.resid) for (int q = 0; q < 3; q++) ra.resid[(size_t)inst * 3 + q] = r1.r[q];
+    }
+    if (t == 0) ra.flags[inst] = accept ? 1 : 0;
+#else
     if constexpr (JVP) {   // ---- solution tangents: dx = z_x - x z_tau, dy = D z_y - y z_tau, ds = D z_y - z_y - s z_tau ----
       apply_D(S, M, M.X + n, M.t2);
       const double zt = M.X[N - 1];
@@ -616,6 +779,7 @@ __global__ void __launch_bounds__(SMALL ? 256 : 512, SMALL ? 4 : 1) BWD_KERNEL(c
       }
       if (t == 0 && a.lsqr_iters) a.lsqr_iters[inst] = itn;
     }
+#endif
     __syncthreads();
   }
 }
@@ -630,7 +794,14 @@ static const void *lsqr_kernel(int dense, int small_cta, int vals_global) {
   if (small_cta) return dense ? (const void *)BWD_KERNEL<true, true, JVP> : (const void *)BWD_KERNEL<false, true, JVP>;
   return dense ? (const void *)BWD_KERNEL<true, false, JVP> : (const void *)BWD_KERNEL<false, false, JVP>;
 }
-#ifndef BC_LSMR
+#if defined(BC_REFINE)
+extern "C" size_t bc_refine_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp,
+                                       int vec_global, int vals_global) {
+  return bwd_smem_doubles(n, m, npoly, nnzA, nnzP_smem, threads, max_psd, psd_total, nexp, vec_global, vals_global, 0, 1) * sizeof(double);
+}
+extern "C" size_t bc_refine_ws_doubles(int n, int m, int npoly) { return (bwd_vec_doubles(n, m, npoly, 0, 1) + 1) & ~(size_t)1; }
+extern "C" const void *bc_refine_kernel(int dense, int small_cta, int vals_global) { return lsqr_kernel<true>(dense, small_cta, vals_global); }
+#elif !defined(BC_LSMR)
 extern "C" size_t bc_bwd_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
                                     int vals_global, int lsmr) {
   return bwd_smem_doubles(n, m, npoly, nnzA, nnzP_smem, threads, max_psd, psd_total, nexp, vec_global, vals_global, lsmr) * sizeof(double);

@@ -130,6 +130,16 @@ struct PolishArgs {
   int refine;            // iterative refinement steps
 };
 
+// Solution refinement (refine.cu, bcone_refine): the forward-mode kernel's arguments (x, y, s read through a.x / a.y / a.s and, for
+// an accepted instance, written through a.tx / a.ty / a.ts: the same arrays) and the refinement's own.
+struct RefineArgs {
+  BwdArgs a;
+  const int *status;
+  int *flags;            // [B]: 1 accepted, 0 rejected (input kept), -1 not attempted
+  double *resid;         // [B,3] or NULL: rp, rd, gap of an accepted instance
+  int steps;             // at most this many Newton steps
+};
+
 // Per-instance record of the shared-matrix adjoint: [r_x n | r_y m | r_tau | pi_y m].
 __host__ __device__ inline long long bc_srec_doubles(int n, int m) { return (long long)n + 2LL * m + 1; }
 // Written by the whole block; rx / ry / piy in shared memory (rx and ry may be one vector X = [r_x ; r_y ; r_tau]).
@@ -1636,6 +1646,11 @@ const void *bc_bwdb_kernel(int lsmr);
 const void *bc_lsmr_kernel(int dense, int small_cta, int jvp, int vals_global);
 const void *bc_bwdf_lsmr_kernel(int n);
 const void *bc_bwdb_lsmr_kernel(void);
+// refine.cu (bwd.cu compiled with BC_REFINE)
+size_t bc_refine_smem_bytes(int n, int m, int npoly, int nnzA, int nnzP_smem, int threads, int max_psd, int psd_total, int nexp, int vec_global,
+                            int vals_global);
+size_t bc_refine_ws_doubles(int n, int m, int npoly);
+const void *bc_refine_kernel(int dense, int small_cta, int vals_global);
 // polish.cu
 size_t bc_polish_smem_bytes(int n, int m, int threads, long long stage_cap);
 const void *bc_polish_kernel(int dense);

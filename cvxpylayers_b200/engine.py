@@ -27,7 +27,7 @@ _ARG_MAP = {
     "acceleration_lookback": "acceleration_lookback", "acceleration_interval": "acceleration_interval",
 }
 _IGNORED = {"verbose", "n_jobs_forward", "n_jobs_backward", "solve_method", "warm_starts", "raise_on_error", "warm_start", "reuse_setup", "shared_matrices",
-            "polish"}   # (warm_start / reuse_setup / shared_matrices / polish are handled by the layer)
+            "polish", "refine"}   # (warm_start / reuse_setup / shared_matrices / polish / refine are handled by the layer)
 
 
 def make_settings(args: dict | None) -> _lib.BconeSettings:
@@ -455,4 +455,49 @@ class Engine:
         rc = fn(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c), _ptr(sol.x), _ptr(sol.y),
                 _ptr(sol.s), _ptr(sol.status), _ptr(flags), _ptr(sol.resid), C.byref(settings), self._stream())
         self._raise(rc, "bcone_polish_shared" if shared else "bcone_polish")
+        return flags
+
+    def require_refine(self) -> None:
+        """Raise ValueError (naming the reason) unless the structure has a refinement plan (``bcone_refine_supported``); no device
+        work, so a layer can refuse the option before it solves anything."""
+        if self.lib.bcone_refine_supported(self.h) != 0:
+            raise ValueError(self.lib.bcone_last_error(self.h).decode())
+
+    def refine_info(self) -> dict:
+        """The refinement plan (``bcone_refine_info``): threads, ctas_per_sm, small_ctas_per_sm (0: no 4-CTA/SM build),
+        vals_global, vec_global, num_sms, and last_small (the build the last refine launch took: 1 the 4-CTA/SM one, -1 none yet)."""
+        v = [C.c_int32() for _ in range(7)]
+        self.lib.bcone_refine_info(self.h, *[C.byref(x) for x in v])
+        k = ["threads", "ctas_per_sm", "small_ctas_per_sm", "vals_global", "vec_global", "num_sms", "last_small"]
+        return {a: int(b.value) for a, b in zip(k, v)}
+
+    def refine(self, A_vals, b, c, sol: Solution, P_vals=None, settings: _lib.BconeSettings | None = None, steps: int = 3) -> torch.Tensor:
+        """Refine ``sol`` in place (``bcone_refine``, include/bcone.h): for each SOLVED / INACCURATE instance take up to ``steps``
+        (1 ... 10) Gauss-Newton steps on the homogeneous embedding's residual map with a backtracking line search, and keep the
+        result only where no residual (primal, dual, gap) grows; ``sol.resid`` is updated for those.  Statuses are not changed.
+        The inner LSQR takes the settings' lsqr_* values (lsqr_precond 2 runs as 1).  Returns refined[B] (int32): 1 accepted,
+        0 rejected (input kept), -1 not attempted.  1-D ``A_vals[nnzA]`` (and ``P_vals[nnzP]``): one copy shared by the batch
+        (``bcone_refine_shared``)."""
+        st, dev, f64 = self.structure, self.device, torch.float64
+        if isinstance(steps, bool) or not isinstance(steps, int) or not 1 <= steps <= 10:
+            raise ValueError(f"refine: steps must be an int in 1 ... 10, got {steps!r}")
+        shared = A_vals.dim() == 1
+        B = b.shape[0] if shared else A_vals.shape[0]
+        lead = () if shared else (B,)
+        for name, t, shp in (("A_vals", A_vals, (*lead, st.nnzA)), ("b", b, (B, st.m)), ("c", c, (B, st.n)),
+                             ("x", sol.x, (B, st.n)), ("y", sol.y, (B, st.m)), ("s", sol.s, (B, st.m))):
+            _chk(t, shp, f64, dev, name)
+        _chk(sol.status, (B,), torch.int32, dev, "status")
+        _chk(sol.resid, (B, 3), f64, dev, "resid")
+        if st.nnzP:
+            if P_vals is None:
+                raise ValueError("structure has a quadratic term but P_vals is None")
+            _chk(P_vals, (*lead, st.nnzP), f64, dev, "P_vals")
+        self.require_refine()
+        settings = settings or _lib.default_settings()
+        flags = torch.empty(B, dtype=torch.int32, device=dev)
+        fn = self.lib.bcone_refine_shared if shared else self.lib.bcone_refine
+        rc = fn(self.h, C.c_int32(B), _ptr(A_vals), _ptr(P_vals if st.nnzP else None), _ptr(b), _ptr(c), _ptr(sol.x), _ptr(sol.y),
+                _ptr(sol.s), _ptr(sol.status), _ptr(flags), _ptr(sol.resid), C.c_int32(steps), C.byref(settings), self._stream())
+        self._raise(rc, "bcone_refine_shared" if shared else "bcone_refine")
         return flags

@@ -323,8 +323,29 @@ def _side_streams(eng: Engine, dev):
     return ss
 
 
+def _post_options(eng: Engine, merged: dict) -> tuple[bool, int]:
+    """The layer options ``polish`` and ``refine`` -> (polish, refinement steps; 0 = off), refused (ValueError) before anything
+    is staged or solved: both at once, a ``refine`` other than a bool or an int in 1 ... 10 (True = 3 steps), or a structure
+    without the plan the option needs."""
+    polish, refine = bool(merged.get("polish")), merged.get("refine", False)
+    if refine is None or refine is False:
+        refine = 0
+    elif refine is True:
+        refine = 3
+    elif not isinstance(refine, (int, np.integer)) or not 1 <= int(refine) <= 10:
+        raise ValueError(f"refine: expected True or an int in 1 ... 10, got {refine!r}")
+    refine = int(refine)
+    if polish and refine:
+        raise ValueError("the layer options polish and refine exclude each other")
+    if polish:
+        eng.require_polish()
+    if refine:
+        eng.require_refine()
+    return polish, refine
+
+
 def _forward_pipelined(eng: Engine, dev, A_eval, q_eval, P_eval, settings, use_P, warm=None, cache=None, staged: bool = False,
-                       polish: bool = False):
+                       polish: bool = False, refine: int = 0):
     st = eng.structure
     B = A_eval.shape[1]
     cstride = (cache.numel() // B) if cache is not None else 0
@@ -380,7 +401,7 @@ def _forward_pipelined(eng: Engine, dev, A_eval, q_eval, P_eval, settings, use_P
             return out
 
         futs = [sg.pool.submit(stage, k, lo, hi) for k, (lo, hi) in enumerate(chunks)]
-    try:   # any exception leaving the chunk loop (a failed copy, solve or polish) releases the stager
+    try:   # any exception leaving the chunk loop (a failed copy, solve, polish or refinement) releases the stager
         for k, (lo, hi) in enumerate(chunks):
             with torch.cuda.stream(streams[k % 2]):
                 Bc = hi - lo
@@ -409,6 +430,8 @@ def _forward_pipelined(eng: Engine, dev, A_eval, q_eval, P_eval, settings, use_P
                           cache=None if cache is None else cache[lo * cstride:hi * cstride], reuse=True)
                 if polish:
                     eng.polish(A_vals[lo:hi], b[lo:hi], c[lo:hi], sol_c, P_vals[lo:hi] if use_P else None, settings)
+                if refine:
+                    eng.refine(A_vals[lo:hi], b[lo:hi], c[lo:hi], sol_c, P_vals[lo:hi] if use_P else None, settings, refine)
                 primal[lo:hi].copy_(sol.x[lo:hi], non_blocking=True)
                 dual[lo:hi].copy_(sol.y[lo:hi], non_blocking=True)
     except BaseException:
@@ -488,22 +511,22 @@ class _CvxpyLayer(torch.autograd.Function):
         piped = _pipe_ok(eng, batch_size, A_eval.detach(), q_eval.detach(), P_eval.detach() if use_P else None)
         staged = (not piped) and eng.kernel_info()["fwd_smem"] > 0 and _stage_ok(batch_size, A_eval, q_eval, P_eval if use_P else None)
         piped = piped or staged
-        # polish: the solution is polished right after the solve, so the backward, the forward mode and the next warm start all
-        # see the polished point
-        polish = bool(merged.get("polish"))
-        if polish:
-            eng.require_polish()   # (before any chunk is staged or solved)
+        # polish / refine: the solution is polished or refined right after the solve, so the backward, the forward mode and the
+        # next warm start all see that point
+        polish, refine = _post_options(eng, merged)   # (before any chunk is staged or solved)
         with torch.cuda.device(dev):
             if piped:
                 A_vals, P_vals, b, c, sol, primal, dual = _forward_pipelined(
                     eng, dev, A_eval.detach(), q_eval.detach(), P_eval.detach() if use_P else None, settings, use_P, warm, cache, staged,
-                    polish)
+                    polish, refine)
             else:
                 A_vals, P_vals, b, c = eng.ingest(_to_dev(A_eval, dev), _to_dev(q_eval, dev),
                                                   _to_dev(P_eval, dev) if use_P else None)
                 sol = eng.solve(A_vals, b, c, P_vals, settings, warm=warm, cache=cache, reuse=True)
                 if polish:
                     eng.polish(A_vals, b, c, sol, P_vals, settings)
+                if refine:
+                    eng.refine(A_vals, b, c, sol, P_vals, settings, refine)
             status = sol.status.cpu()  # the one host sync of the forward: per-instance status
         ctx.remember(dev, batch_size, sol, merged, warm_start)
         bad = (status != 1) & (status != 2)
@@ -634,14 +657,16 @@ class _CvxpyLayerFused(torch.autograd.Function):
         # shared_matrices: the caller states that A and P are the same for every instance (their parameters are unbatched);
         # they are evaluated once and the batch shares them through solve, adjoint and forward mode
         shared = bool(merged.get("shared_matrices"))
-        if merged.get("polish"):
-            eng.require_polish()
+        polish, refine = _post_options(eng, merged)
         with torch.cuda.device(dev):
             cache = ctx.setup_cache(eng, dev, B, merged)
             A_vals, P_vals, b, c = eng.ingest_params(_to_dev(ps, dev), shared=shared)
             sol = eng.solve(A_vals, b, c, P_vals, settings, warm=ctx.warm_for(dev, B, warm_start, merged), cache=cache, reuse=True)
-            if merged.get("polish"):   # (before the solution is kept for the backward, the forward mode and the next warm start)
+            # (before the solution is kept for the backward, the forward mode and the next warm start)
+            if polish:
                 eng.polish(A_vals, b, c, sol, P_vals, settings)
+            if refine:
+                eng.refine(A_vals, b, c, sol, P_vals, settings, refine)
             status = sol.status.cpu()
         ctx.remember(dev, B, sol, merged, warm_start)
         bad = (status != 1) & (status != 2)

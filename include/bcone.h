@@ -286,6 +286,37 @@ int bcone_polish_shared(void *handle, int32_t B, const double *A_vals, const dou
                         double *x, double *y, double *s, const int32_t *status, int32_t *polished, double *resid,
                         const bcone_settings *st, void *cuda_stream);
 
+/* Solution refinement (Busseti, Moursi & Boyd 2019) for every cone type: Gauss-Newton on the homogeneous embedding's residual
+ * map at tau = 1.  For every instance whose status is SOLVED (1) or INACCURATE (2), from w = (x, v = y - s), pi = Pi_{K*}(v):
+ *   R(x, v) = [P x + A'pi + c ;  b - A x - (pi - v) ;  -(x'P x + c'x + b'pi)],
+ * a step solves min ||J z + R|| (J = the first n + m columns of the forward mode's derivative matrix, the tau column masked) by
+ * LSQR with the settings' lsqr_atol / btol / conlim / iter_lim and lsqr_precond 0 or 1 (2 runs as 1; settings.lsmr does not
+ * apply), then takes the first of alpha = 1, 1/2, ..., 1/32 with a smaller ||R(w + alpha z)||_2 (none: stop); at most `steps`
+ * steps (1 ... 10).  The candidate x, y = pi, s = pi - v (y in K*, s in K, y's = 0 exactly) replaces the input only when none
+ * of polishing's rp, rd, gap (bcone_polish) exceeds the input's.  THE STATUS IS NEVER CHANGED.
+ *   x[B,n], y[B,m], s[B,m]: read, and overwritten for accepted instances only (a rejected one keeps its bits);
+ *   status[B]: the forward's; refined[B] (int32, out): 1 accepted, 0 rejected (input kept), -1 not attempted (other status or
+ *   a non-finite x / y / s); resid[B,3] or NULL: rp, rd, gap, updated for accepted instances.
+ * No atomics: results are deterministic.  BCONE_EINVAL for steps outside 1 ... 10; BCONE_EUNSUPPORTED (message: why) for a
+ * structure without a refinement plan.  bcone_refine_shared: A_vals[nnzA] / P_vals[nnzP] one copy for the batch; the same
+ * bits as bcone_refine on the expanded copies. */
+int bcone_refine(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                 double *x, double *y, double *s, const int32_t *status, int32_t *refined, double *resid, int32_t steps,
+                 const bcone_settings *st, void *cuda_stream);
+/* BCONE_OK when the structure has a refinement plan, else BCONE_EUNSUPPORTED with the reason in bcone_last_error(handle).
+ * No device work. */
+int bcone_refine_supported(void *handle);
+/* The refinement plan (all 0 without one): threads and resident CTAs per SM of its 128-register (or 512-thread) build, CTAs
+ * per SM of its 4-CTA/SM build (0: none), whether the values are read off chip and the vectors kept in a global slab, the
+ * device's SM count, and which build the last bcone_refine launch took (1 the 4-CTA/SM build, 0 the other, -1 no launch yet;
+ * a launch takes the 4-CTA/SM build when the batch exceeds what the other keeps resident, or always with BCONE_SMALL_CTA=2).
+ * Any pointer may be NULL.  No device work. */
+int bcone_refine_info(void *handle, int32_t *threads, int32_t *ctas_per_sm, int32_t *small_ctas_per_sm, int32_t *vals_global,
+                      int32_t *vec_global, int32_t *num_sms, int32_t *last_small);
+int bcone_refine_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
+                        double *x, double *y, double *s, const int32_t *status, int32_t *refined, double *resid, int32_t steps,
+                        const bcone_settings *st, void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
