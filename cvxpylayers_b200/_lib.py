@@ -22,7 +22,7 @@ EXPORTS = [
     "bcone_peer_free", "bcone_copy2d_async", "bcone_rows_from_param", "bcone_param_from_rows", "bcone_gather_cols", "bcone_scatter_cols", "bcone_set_param_maps", "bcone_ingest_params", "bcone_emit_params", "bcone_solve", "bcone_solve_warm", "bcone_solve_cached", "bcone_cache_bytes", "bcone_vjp", "bcone_jvp", "bcone_launch_count", "bcone_fallback_count", "bcone_kernel_info", "bcone_path_info", "bcone_small_cta_info", "bcone_memcpy2d", "bcone_set_profile",
     "bcone_solve_shared", "bcone_vjp_shared", "bcone_jvp_shared", "bcone_ingest_params_shared", "bcone_emit_params_shared",
     "bcone_polish", "bcone_polish_shared", "bcone_polish_supported", "bcone_refine", "bcone_refine_shared", "bcone_refine_supported",
-    "bcone_refine_info",
+    "bcone_refine_info", "bcone_polish_info",
 ]
 
 
@@ -136,6 +136,8 @@ def load() -> C.CDLL:
     lib.bcone_polish_shared.restype = C.c_int
     lib.bcone_polish_supported.argtypes = [vp]
     lib.bcone_polish_supported.restype = C.c_int
+    lib.bcone_polish_info.argtypes = [vp] + [_i32p] * 3 + [C.POINTER(C.c_int64)]
+    lib.bcone_polish_info.restype = C.c_int
     lib.bcone_refine.argtypes = [vp, C.c_int32] + [vp] * 10 + [C.c_int32, C.POINTER(BconeSettings), vp]
     lib.bcone_refine.restype = C.c_int
     lib.bcone_refine_shared.argtypes = [vp, C.c_int32] + [vp] * 10 + [C.c_int32, C.POINTER(BconeSettings), vp]

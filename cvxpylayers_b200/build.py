@@ -18,7 +18,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 SOURCES = ["api.cu", "fwd.cu", "fwd_fast.cu", "bwd.cu", "bwd_fast.cu", "bwd_block.cu", "bwd_lsmr.cu", "bwd_fast_lsmr.cu", "bwd_block_lsmr.cu",
-           "pack.cu", "shared.cu", "polish.cu", "refine.cu"]
+           "pack.cu", "shared.cu", "polish.cu", "polish_large.cu", "refine.cu"]
 HEADERS = [CSRC / "common.cuh", PKG.parent / "include" / "bcone.h"]
 LIB = PKG / "libbcone.so"
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]

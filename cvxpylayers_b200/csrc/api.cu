@@ -82,10 +82,14 @@ struct Handle {
   Plan fwd_fast;    // fast_fwd: dense A, polyhedral cones, direct mode: register-tiled forward (fwd_fast.cu)
   int fast_fwd = 0;
   LsPlans ls[2];
-  // solution polishing (polish.cu): planned only for zero + nonneg cones, n <= 128, when it fits; otherwise polish_why says why
+  // solution polishing: planned only for zero + nonneg cones; otherwise polish_why says why.  Tier 0 (polish.cu): on chip, for
+  // n <= 128 when it fits; tier 1 (polish_large.cu): everything else, with each CTA's working set in a slab of global memory.
   Plan polish;
-  int polish_ok = 0;
-  long long polish_stage = 0;   // doubles of its staging buffer (live rows of A, then W and S)
+  int polish_ok = 0, polish_tier = -1;
+  long long polish_stage = 0;   // tier 0: doubles of its staging buffer (live rows of A, then W and S)
+  long long polish_slab = 0;    // tier 1: doubles of slab per CTA
+  int polish_ctas = 0;          // tier 1: CTAs of the grid (the SM count, fewer when the slabs would exceed the budget)
+  int p_diag = 1;               // no P, or only diagonal entries (the slab tier's L_P is then a vector)
   std::string polish_why;
   // solution refinement (refine.cu): the forward mode's tiers with the refinement kernel's sizes; refine_why when it does not fit
   TieredPlan refine;
@@ -98,7 +102,7 @@ struct Handle {
   // srec / part = the adjoint's per-instance r, pi_y records and the reduction's partial sums (shared.cu)
   // bwd / jvp: the generic backward's vector slabs, per least-squares method
   struct StreamWs { cudaStream_t s; double *fwd = nullptr, *aa = nullptr, *park = nullptr; size_t aa_cap = 0;
-                    double *bwd[2] = {nullptr, nullptr}, *jvp[2] = {nullptr, nullptr}, *refine = nullptr;
+                    double *bwd[2] = {nullptr, nullptr}, *jvp[2] = {nullptr, nullptr}, *refine = nullptr, *polish = nullptr;
                     double *setup = nullptr, *srec = nullptr, *part = nullptr; size_t srec_cap = 0, part_cap = 0; };
   std::vector<StreamWs> sws;
   int *fail_list[RING] = {nullptr}; int fail_cap[RING] = {0};
@@ -234,7 +238,7 @@ void analyse_and_upload(Handle *h, const bcone_desc *d) {
   S.cone_type = upload(h, ctype); S.cone_start = upload(h, cstart); S.cone_size = upload(h, csize); S.cone_order = upload(h, corder);
   if (S.nnzP > 0) {
     std::vector<int> pptr(d->P_indptr, d->P_indptr + n + 1), pidx(d->P_indices, d->P_indices + S.nnzP), prow(S.nnzP);
-    for (int i = 0; i < n; i++) for (int k = pptr[i]; k < pptr[i + 1]; k++) prow[k] = i;
+    for (int i = 0; i < n; i++) for (int k = pptr[i]; k < pptr[i + 1]; k++) { prow[k] = i; if (pidx[k] != i) h->p_diag = 0; }
     S.P_indptr = upload(h, pptr); S.P_indices = upload(h, pidx); S.P_rowof = upload(h, prow);
     // CSC view of the upper triangle + dense-pattern detection (row-major full upper triangle)
     std::vector<int> pc(n + 1, 0), pr(S.nnzP), pp(S.nnzP);
@@ -380,28 +384,49 @@ int plan_backward(Handle *h, const Limits &L, int lsmr) {
   return rc;
 }
 
-// Solution polishing: zero + nonneg cones (a finite active set) and n <= 128 (W = L^{-1} A_L' is formed with 8 rows of A in a
-// warp's registers).  The staging buffer holds the live rows (at most min(m, n)), then W and S; it is as large as that needs
-// or as what is left of the opt-in shared memory, and an instance whose W and S do not fit it is not attempted.  Sets
-// h->polish_ok, or h->polish_why.  Never fails bcone_create.
+// Solution polishing, slab tier: one 512-thread CTA per SM, each with a slab of global memory for the instance's live rows,
+// vectors, L_P^{-1}, W and S (bc_polish_large_slab_doubles).  The slabs of the grid stay within min(4 GB, half the device memory
+// free at bcone_create): fewer CTAs when they would not, no plan when one slab alone would not.
+void plan_polish_slab(Handle *h) {
+  const DevStruct &S = h->S;
+  const int tt = bc_polish_large_threads();
+  const long long per = bc_polish_large_slab_doubles(S.n, S.m, tt, h->p_diag);
+  size_t free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
+  const size_t budget = std::min((size_t)4 << 30, free_b / 2), bytes = (size_t)per * sizeof(double);
+  if (bytes > budget) {
+    h->polish_why = "polish: the working set of one instance needs " + std::to_string(bytes) + " B of global memory, more than the budget of " +
+                    std::to_string(budget) + " B (min(4 GB, half the free device memory))";
+    return;
+  }
+  Plan p{bc_polish_large_kernel(S.dense), tt, bc_polish_large_smem_bytes(tt)};
+  if (configure(p) != cudaSuccess) { h->polish_why = "polish: kernel configuration failed"; return; }
+  h->polish = p; h->polish_ok = 1; h->polish_tier = 1; h->polish_slab = per;
+  h->polish_ctas = (int)std::max<size_t>(1, std::min<size_t>((size_t)h->num_sms * p.ctas, budget / bytes));
+}
+
+// Solution polishing: zero + nonneg cones (a finite active set).  On chip (polish.cu) for n <= 128 (W = L^{-1} A_L' is formed
+// with 8 rows of A in a warp's registers): the staging buffer holds the live rows (at most min(m, n)), then W and S; it is as
+// large as that needs or as what is left of the opt-in shared memory, and an instance whose W and S do not fit it is not
+// attempted.  Every other such structure takes the slab tier.  Sets h->polish_ok, or h->polish_why.  Never fails bcone_create.
 void plan_polish(Handle *h, const Limits &L) {
   const DevStruct &S = h->S;
   const int n = S.n, m = S.m;
   if (S.ncones > 0 || S.ep + S.ed > 0) { h->polish_why = "polish: only structures with zero and nonneg cones have a finite active set to polish (this one has SOC, PSD or exponential cones)"; return; }
-  if (n > 128) { h->polish_why = "polish: needs n <= 128 (n = " + std::to_string(n) + ")"; return; }
-  const long long k = std::min(m, n), full = k * n + k * (k + 1) / 2;
-  for (int tt = L.threads; tt >= 128; tt /= 2) {
-    const size_t base = bc_polish_smem_bytes(n, m, tt, 0);
-    if (base > L.smem_cap) continue;
-    const long long cap = std::min(full, (long long)((L.smem_cap - base) / sizeof(double)) & ~1LL);
-    if (cap < std::min(full, (long long)n + 1)) continue;   // (not even one live row)
-    h->polish = Plan{bc_polish_kernel(S.dense), tt, bc_polish_smem_bytes(n, m, tt, cap)};
-    if (configure(h->polish) != cudaSuccess) { h->polish_why = "polish: kernel configuration failed"; return; }
-    h->polish_ok = 1; h->polish_stage = cap;
-    return;
+  if (n <= 128) {
+    const long long k = std::min(m, n), full = k * n + k * (k + 1) / 2;
+    for (int tt = L.threads; tt >= 128; tt /= 2) {
+      const size_t base = bc_polish_smem_bytes(n, m, tt, 0);
+      if (base > L.smem_cap) continue;
+      const long long cap = std::min(full, (long long)((L.smem_cap - base) / sizeof(double)) & ~1LL);
+      if (cap < std::min(full, (long long)n + 1)) continue;   // (not even one live row)
+      h->polish = Plan{bc_polish_kernel(S.dense), tt, bc_polish_smem_bytes(n, m, tt, cap)};
+      if (configure(h->polish) != cudaSuccess) { h->polish_why = "polish: kernel configuration failed"; return; }
+      h->polish_ok = 1; h->polish_stage = cap; h->polish_tier = 0;
+      return;
+    }
   }
-  h->polish_why = "polish: does not fit in shared memory (" + std::to_string(bc_polish_smem_bytes(n, m, 128, std::min(full, (long long)n + 1))) +
-                  " B needed, " + std::to_string(L.smem_cap) + " B per CTA available)";
+  plan_polish_slab(h);
 }
 
 // Solution refinement: the forward mode's tier search with the refinement kernel's sizes (every cone type has one).  Sets
@@ -973,8 +998,16 @@ static int polish_impl(Handle *h, int32_t B, const double *A_vals, const double 
   a.delta = 1e-6; a.refine = 3;   // OSQP's defaults
   int *ctr = h->counters + 4 * (h->slot++ % Handle::RING);
   a.counter = ctr;
+  PolishLargeArgs g{};
+  if (h->polish_tier == 1) {
+    Handle::StreamWs *sw = stream_ws(h, st);
+    if (!ensure_slab(h, &sw->polish, nullptr, (size_t)h->polish_slab * h->polish_ctas)) return fail(h, BCONE_ENOMEM, "cudaMalloc polish workspace");
+    a.use_tma = 0; a.stage_cap = 0;
+    g.a = a; g.ws = sw->polish; g.ws_stride = h->polish_slab; g.p_diag = h->p_diag;
+  }
   CK(cudaMemsetAsync(ctr, 0, sizeof(int), st), "polish counter");
-  CK(launch(h->polish, grid_for(h->polish, B, h->num_sms), &a, st), "polish launch");
+  if (h->polish_tier == 1) CK(launch(h->polish, std::min(B, h->polish_ctas), &g, st), "polish launch (slab)");
+  else CK(launch(h->polish, grid_for(h->polish, B, h->num_sms), &a, st), "polish launch");
   h->launches++;
   return BCONE_OK;
 }
@@ -982,6 +1015,16 @@ extern "C" int bcone_polish_supported(void *handle) {
   Handle *h = (Handle *)handle;
   if (!h) return BCONE_EINVAL;
   return h->polish_ok ? BCONE_OK : fail(h, BCONE_EUNSUPPORTED, h->polish_why);
+}
+extern "C" int bcone_polish_info(void *handle, int32_t *tier, int32_t *threads, int32_t *ctas, int64_t *slab_bytes_per_cta) {
+  Handle *h = (Handle *)handle;
+  if (!h) return BCONE_EINVAL;
+  const int tr = h->polish_ok ? h->polish_tier : -1;
+  if (tier) *tier = tr;
+  if (threads) *threads = tr >= 0 ? h->polish.threads : 0;
+  if (ctas) *ctas = tr == 1 ? h->polish_ctas : (tr == 0 ? h->num_sms * h->polish.ctas : 0);
+  if (slab_bytes_per_cta) *slab_bytes_per_cta = tr == 1 ? (int64_t)h->polish_slab * (int64_t)sizeof(double) : 0;
+  return BCONE_OK;
 }
 extern "C" int bcone_polish(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c, double *x,
                             double *y, double *s, const int32_t *status, int32_t *polished, double *resid, const bcone_settings *st, void *stream) {

@@ -130,6 +130,15 @@ struct PolishArgs {
   int refine;            // iterative refinement steps
 };
 
+// Solution polishing, slab tier (polish_large.cu): polishing's arguments (stage_cap and use_tma unused), each CTA's slab of global
+// memory and the P layout decided at bcone_create.
+struct PolishLargeArgs {
+  PolishArgs a;
+  double *ws;            // per-CTA slabs, ws_stride doubles apart (bc_polish_large_slab_doubles)
+  long long ws_stride;
+  int p_diag;            // no P, or only diagonal entries: L_P is the vector sqrt(P_jj + d), W is A_L with its columns scaled
+};
+
 // Solution refinement (refine.cu, bcone_refine): the forward-mode kernel's arguments (x, y, s read through a.x / a.y / a.s and, for
 // an accepted instance, written through a.tx / a.ty / a.ts: the same arrays) and the refinement's own.
 struct RefineArgs {
@@ -1654,6 +1663,11 @@ const void *bc_refine_kernel(int dense, int small_cta, int vals_global);
 // polish.cu
 size_t bc_polish_smem_bytes(int n, int m, int threads, long long stage_cap);
 const void *bc_polish_kernel(int dense);
+// polish_large.cu (the slab tier of polishing)
+long long bc_polish_large_slab_doubles(int n, int m, int threads, int p_diag);
+size_t bc_polish_large_smem_bytes(int threads);
+int bc_polish_large_threads(void);
+const void *bc_polish_large_kernel(int dense);
 // pack.cu
 cudaError_t bc_b2e(const double *in, double *out, int K, int B, int ldo, int roff, const int *smap, const int *dmap, double sign, long long ldb,
                    cudaStream_t st);

@@ -434,7 +434,9 @@ class Engine:
         of the active set its iterate identifies and keep the result only where no residual (primal, dual, gap) grows; ``sol.resid``
         is updated for those.  Statuses are not changed.  Returns polished[B] (int32): 1 accepted, 0 rejected (input kept),
         -1 not attempted.  1-D ``A_vals[nnzA]`` (and ``P_vals[nnzP]``): one copy shared by the batch (``bcone_polish_shared``).
-        Structures with other than zero and nonneg cones, or n > 128, raise ValueError."""
+        Any n: structures with n <= 128 that fit in shared memory polish on chip, the others in a slab of global memory per CTA
+        (``polish_info``).  Structures with other than zero and nonneg cones, or whose one-instance slab exceeds the memory budget,
+        raise ValueError."""
         st, dev, f64 = self.structure, self.device, torch.float64
         shared = A_vals.dim() == 1
         B = b.shape[0] if shared else A_vals.shape[0]
@@ -456,6 +458,14 @@ class Engine:
                 _ptr(sol.s), _ptr(sol.status), _ptr(flags), _ptr(sol.resid), C.byref(settings), self._stream())
         self._raise(rc, "bcone_polish_shared" if shared else "bcone_polish")
         return flags
+
+    def polish_info(self) -> dict:
+        """The polish plan (``bcone_polish_info``): tier (0 on chip, 1 slab of global memory, -1 no plan), threads, ctas (the most
+        CTAs a launch runs) and slab_bytes_per_cta (0 on chip)."""
+        v = [C.c_int32() for _ in range(3)]
+        slab = C.c_int64()
+        self.lib.bcone_polish_info(self.h, *[C.byref(x) for x in v], C.byref(slab))
+        return {"tier": int(v[0].value), "threads": int(v[1].value), "ctas": int(v[2].value), "slab_bytes_per_cta": int(slab.value)}
 
     def require_refine(self) -> None:
         """Raise ValueError (naming the reason) unless the structure has a refinement plan (``bcone_refine_supported``); no device

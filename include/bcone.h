@@ -262,7 +262,7 @@ int bcone_path_info(void *handle, int32_t *fwd_path, int32_t *bwd_path);
  * that build takes it. */
 int bcone_small_cta_info(void *handle, int32_t *fwd_small_ctas, int32_t *bwd_small_ctas);
 
-/* Solution polishing (OSQP's `polish`) for QPs and LPs whose cones are zero and nonneg only, n <= 128.  For every instance
+/* Solution polishing (OSQP's `polish`) for QPs and LPs whose cones are zero and nonneg only, any n.  For every instance
  * whose status is SOLVED (1) or INACCURATE (2): the live rows L are the zero rows and the nonneg rows with y_i > s_i; the
  * equality-constrained QP of L is solved through [[P + d I, A_L'], [A_L, -d I]] (d = 1e-6 x the largest absolute entry of P
  * and A_L) and three steps of iterative refinement against the unregularised KKT matrix; the point is completed with y = 0
@@ -270,21 +270,29 @@ int bcone_small_cta_info(void *handle, int32_t *fwd_small_ctas, int32_t *bwd_sma
  * rp = |Ax + s - b|_inf, rd = |Px + A'y + c|_inf, gap = |x'Px + c'x + b'y| exceeds the input's.  THE STATUS IS NEVER CHANGED.
  *   x[B,n], y[B,m], s[B,m]: read, and overwritten for accepted instances only (a rejected one keeps its bits);
  *   status[B]: the forward's; polished[B] (int32, out): 1 accepted, 0 rejected (input kept; also when P + d I or the Schur
- *   complement is not positive definite), -1 not attempted (other status, a non-finite x / y / s, or more live rows than
- *   n or than the staging buffer holds); resid[B,3] or NULL: rp, rd, gap, updated for accepted instances.  `st` is taken for
- *   symmetry with the other entry points; polishing has no setting (d and the refinement count are fixed).
- * No atomics: results are deterministic.  BCONE_EUNSUPPORTED (message: the cone types, n, or the shared memory) for a
- * structure without a polish plan.  bcone_polish_shared: A_vals[nnzA] / P_vals[nnzP] one copy for the batch; the same bits
- * as bcone_polish on the expanded copies. */
+ *   complement is not positive definite), -1 not attempted (other status, a non-finite x / y / s, more live rows than n, or,
+ *   on chip, more than the staging buffer holds); resid[B,3] or NULL: rp, rd, gap, updated for accepted instances.  `st` is
+ *   taken for symmetry with the other entry points; polishing has no setting (d and the refinement count are fixed).
+ * Two tiers, chosen at bcone_create from the structure (bcone_polish_info): on chip for n <= 128 when the instance fits in
+ * shared memory, else a slab of global memory per CTA of min(m, n) x n + min(m, n)^2 / 2 doubles (+ n^2 / 2 with an
+ * off-diagonal P), with the grid's slabs within min(4 GB, half the device memory free at bcone_create); the first call on a
+ * stream allocates that stream's slabs.
+ * No atomics: results are deterministic and do not depend on the grid.  BCONE_EUNSUPPORTED (message: the cone types, or the
+ * bytes one instance needs) for a structure without a polish plan.  bcone_polish_shared: A_vals[nnzA] / P_vals[nnzP] one copy
+ * for the batch; the same bits as bcone_polish on the expanded copies. */
 int bcone_polish(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
                  double *x, double *y, double *s, const int32_t *status, int32_t *polished, double *resid,
                  const bcone_settings *st, void *cuda_stream);
-/* BCONE_OK when the structure has a polish plan, else BCONE_EUNSUPPORTED with the reason in bcone_last_error(handle): lets a
- * caller refuse the option before it solves anything.  No device work. */
+/* BCONE_OK when the structure has a polish plan (either tier), else BCONE_EUNSUPPORTED with the reason in
+ * bcone_last_error(handle): lets a caller refuse the option before it solves anything.  No device work. */
 int bcone_polish_supported(void *handle);
 int bcone_polish_shared(void *handle, int32_t B, const double *A_vals, const double *P_vals, const double *b, const double *c,
                         double *x, double *y, double *s, const int32_t *status, int32_t *polished, double *resid,
                         const bcone_settings *st, void *cuda_stream);
+/* The polish plan: tier 0 on chip, 1 slab of global memory, -1 no plan; threads per CTA; ctas: the most CTAs a launch runs
+ * (a smaller batch runs one per instance); slab_bytes_per_cta: the slab tier's global memory per CTA (0 on chip).  Any
+ * pointer may be NULL.  No device work. */
+int bcone_polish_info(void *handle, int32_t *tier, int32_t *threads, int32_t *ctas, int64_t *slab_bytes_per_cta);
 
 /* Solution refinement (Busseti, Moursi & Boyd 2019) for every cone type: Gauss-Newton on the homogeneous embedding's residual
  * map at tau = 1.  For every instance whose status is SOLVED (1) or INACCURATE (2), from w = (x, v = y - s), pi = Pi_{K*}(v):
